@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — env-steps/s of the batched PCT step (BASELINE.json metric) on N B200s of one node.
+"""bench.py — env-steps/s of the batched PCT step (BASELINE.json metric) on N H100s of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--setting S] [--envs-per-gpu E] [--continuous]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--setting S] [--envs-per-gpu E] [--continuous] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is ONE batched environment step over all envs of a rank: the synthetic uniform-valid-leaf policy kernel + the PCT step
@@ -20,6 +20,9 @@ The same JSON line carries the other BASELINE configs as sub-records under `conf
 `vec_env`  : the same metric through the reference-facing VecEnv surface (PctVecEnv.step: device observation, host reward / done / infos).
 `roofline` : HBM roofline of the dominant kernel group, algorithmic bytes per launch (DESIGN.md section 5) / its mean duration measured here
              with CUDA events (second pass with events between the kernels).
+`--dump-outputs DIR`: after the timed steps, what the last timed step returned to its caller (observation, reward, done, info, and the
+             leaf indices it was given) goes to DIR/<name>.npy as float32 / float64; inputs are seeded, so two builds compare output for output.
+             Above DUMP_LIMIT bytes in all, a fixed, seeded sample of env rows is written, with their indices in DIR/env_index.npy.
 `cpu_baseline` / `--impl reference`: the CPU restatement of the reference env (oracle/, C, pthreads over envs like the reference's
              ShmemVecEnv workers) on this box's host cores; >= 3 repeats of >= 1 s each, median reported (min / max beside it).
 """
@@ -38,6 +41,7 @@ ITEM_SET = [(i, j, k) for i in range(1, 6) for j in range(1, 6) for k in range(1
 ITEM_SEED, POLICY_SEED = 1234, 4321
 METRIC = "env-steps/s (batched PCT step)"
 PREROLL = 256  # steps after the synchronised reset before anything is timed: the batch reaches its steady-state episode mix
+DUMP_LIMIT, DUMP_SEED = 64 * 1024 * 1024, 2024  # --dump-outputs: total bytes written, seed of the env-row sample above that
 
 
 def parse():
@@ -54,7 +58,12 @@ def parse():
     ap.add_argument("--skip-configs", action="store_true", help="headline only: no sub-records for the other BASELINE configs")
     ap.add_argument("--continuous", action="store_true", help="BASELINE config 4: PctContinuous, sample_from_distribution, bin 1x1x1")
     ap.add_argument("--preroll", type=int, default=PREROLL)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32 / float64)")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    return a
 
 
 def workload_name(setting, continuous, envs_per_gpu, n_gpus):
@@ -66,7 +75,7 @@ def workload_name(setting, continuous, envs_per_gpu, n_gpus):
 
 # ------------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -114,18 +123,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic():
-    """DRAM bytes per launch of the kernels from the committed ncu captures (profiles/traffic.json: per kernel, with the commit they were taken at)."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -194,10 +192,10 @@ def make_batch(setting, continuous, n, rank, local):
     return pct_b200.PctBatch(n, setting, item_set=ITEM_SET, seed=ITEM_SEED, env_id_base=rank * n, device=local)
 
 
-def measure(cx, setting, continuous, n, K, W, preroll, kernels=True, keep=False):
+def measure(cx, setting, continuous, n, K, W, preroll, kernels=True, keep=False, dump=False):
     """Device-timed throughput of one configuration on this rank's GPU (all ranks call it together): reset, `preroll` + W untimed steps,
     K timed steps (CUDA events per step, L2 flushed before each, barrier on both sides), then — discrete only — a second pass of K steps
-    with events between the kernels for the per-kernel durations."""
+    with events between the kernels for the per-kernel durations.  dump: rec["outputs"] holds host copies of what the last timed step returned."""
     import torch
     batch = make_batch(setting, continuous, n, cx.rank, cx.local)
     batch.reset()
@@ -212,17 +210,28 @@ def measure(cx, setting, continuous, n, K, W, preroll, kernels=True, keep=False)
     t_wall0 = time.perf_counter()
     for t in range(K):
         if cx.flush is not None:
-            cx.flush.zero_()  # L2 flush (256 MiB > 126 MB L2), outside the timed interval of the step
+            cx.flush.zero_()  # L2 flush (256 MiB > 50 MB L2), outside the timed interval of the step
         ev[t][0].record()
         idx = batch.random_policy(POLICY_SEED, T0 + t)
         ev[t][1].record()
-        _, _, _, info = batch.step(leaf_idx=idx)
+        obs, rew, done, info = batch.step(leaf_idx=idx)
         ev[t][2].record()
         if t % 16 == 0:
             stats += torch.stack([info[:, 0].double().mean(), info[:, 5].double().mean(), info[:, 6].double().mean(), info[:, 7].double().mean()])
     cx.barrier()
     wall = time.perf_counter() - t_wall0
     launches = batch.kernel_launches - l0
+    outputs = None
+    if dump:  # copied before the profiling pass below steps the batch again
+        outputs = {"obs": obs.float(), "reward": rew.float(), "done": done.float(), "info": info.double(), "leaf_idx": idx.double()}
+        row_bytes = sum(v[0].numel() * v.element_size() for v in outputs.values())
+        if n * row_bytes > DUMP_LIMIT:  # a fixed, seeded sample of env rows (8 more bytes per row for its index, 4 KB for the .npy headers)
+            import numpy as np
+            sample = np.sort(np.random.default_rng(DUMP_SEED).choice(n, (DUMP_LIMIT - 4096) // (row_bytes + 8), replace=False))
+            rows = torch.as_tensor(sample, device=obs.device)
+            outputs = {k: v.index_select(0, rows) for k, v in outputs.items()}
+            outputs["env_index"] = torch.as_tensor(sample.astype(np.float64))
+        outputs = {k: v.cpu().numpy() for k, v in outputs.items()}
     kms, ksteps = {}, 0
     if kernels and not continuous:
         batch.profile(True)
@@ -251,6 +260,8 @@ def measure(cx, setting, continuous, n, K, W, preroll, kernels=True, keep=False)
            "gpu_launches": int(launches), "mean_boxes": mean_boxes, "mean_ems": mean_ems, "mean_valid_leaves": mean_leaf,
            "mean_candidates": mean_cand, "kernel_ms": {k: v / ksteps for k, v in kms.items()} if ksteps else None, "steps": K, "warmup": W,
            "preroll": preroll, "envs_per_gpu": n}
+    if outputs is not None:
+        rec["outputs"] = outputs
     if per_rank:
         rec["per_rank_ms_per_step"] = per_rank  # value uses the MAX: a launch lasts as long as its heaviest env, and N ranks sample N times more tails
     if keep:
@@ -298,16 +309,6 @@ def roofline_of(rec, setting, continuous, n, obs_len, delta_obs):
     ach_survey = b_survey * n / (rec["kernel_ms_per_step"] * 1e-3) / 1e9
     out["survey_formula"] = {"bytes_per_env_step": b_survey, "achieved": ach_survey, "frac": ach_survey / peak,
                              "note": "SURVEY 8(d): (5593 + 24 N + 48 E) B x env-steps/s of one GPU / peak, whole step"}
-    tr = ncu_traffic()
-    out["traffic"] = None
-    if tr and not continuous:
-        ks = [k for k in tr.get("kernels", {}) if k in out["kernel"]]  # the kernels of the dominant group
-        if ks:
-            out["traffic"] = sum(tr["kernels"][k]["dram_bytes_per_launch"] for k in ks)
-            out["traffic_source"] = "dram__bytes_read + write of %s from the ncu --set full captures of %s (profiles/%s; 4096 envs, setting 1, caches flushed per replay)" % (
-                " + ".join(ks), tr.get("commit"), tr.get("file"))
-        out["traffic_all_kernels"] = {k: v["dram_bytes_per_launch"] for k, v in tr.get("kernels", {}).items()}
-        out["traffic_step_total"] = tr.get("step_total_dram_bytes")
     return out
 
 
@@ -346,8 +347,13 @@ def run_ours(a):
     if sampler:
         sampler.start()
         time.sleep(0.3)
-    head, batch = measure(cx, a.setting, a.continuous, n, K, W, a.preroll, keep=True)
+    head, batch = measure(cx, a.setting, a.continuous, n, K, W, a.preroll, keep=True, dump=a.dump_outputs is not None)
     clocks = sampler.finish() if sampler else None
+    if a.dump_outputs is not None:
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        suffix = "_rank%d" % rank if world > 1 else ""
+        for name, arr in head.pop("outputs").items():
+            np.save(os.path.join(a.dump_outputs, name + suffix + ".npy"), arr)
     ol = batch.obs_len
 
     # ---- e2e: host buffers through pct_step_host, host policy on the returned records ----

@@ -1,4 +1,4 @@
-/* pct_b200 — C ABI of the B200-native batched PCT environment (drop-in boundary).
+/* pct_b200 — C ABI of the H100-native batched PCT environment (drop-in boundary).
  *
  * The reference (alexfrom0815/Online-3D-BPP-PCT @ 5e088f2) has no native interface: its
  * environment is a Python gym.Env (pct_envs/PctDiscrete0/bin3D.py:8-188,
@@ -35,7 +35,7 @@ enum pct_status {
     PCT_OK = 0,
     PCT_ERR_INVALID = -1,   /* bad argument / unsupported configuration            */
     PCT_ERR_CUDA = -2,      /* CUDA runtime error (text in pct_last_error)          */
-    PCT_ERR_NO_DEVICE = -3, /* no usable sm_100 device: the library has NO CPU fallback */
+    PCT_ERR_NO_DEVICE = -3, /* no usable sm_90 device: the library has NO CPU fallback */
     PCT_ERR_STATE = -4      /* call sequence error (e.g. step before reset)         */
 };
 

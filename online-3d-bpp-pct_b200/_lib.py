@@ -45,7 +45,7 @@ EXPORTS = ["pct_create", "pct_destroy", "pct_last_error", "pct_set_item_set", "p
 
 
 def build(verbose=False):
-    """Compile csrc/*.cu for sm_100a into libpct_b200.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into libpct_b200.so (nvcc cross-compiles without a GPU)."""
     subprocess.check_call(["make", "-C", os.path.join(_HERE, "csrc")] + ([] if verbose else ["-s"]))
     return LIB_PATH
 

@@ -1,4 +1,4 @@
-"""PctBatch — N PCT environments living on one B200, stepped by the CUDA kernels behind the C ABI.
+"""PctBatch — N PCT environments living on one H100, stepped by the CUDA kernels behind the C ABI.
 
 PyTorch is used for device buffers and streams only (observation / action / reward tensors); every
 environment computation happens inside libpct_b200.so.  Mirrors the constructor kwargs of the reference's
@@ -24,7 +24,7 @@ class PctBatch(object):
         """shuffle: the reference's `shuffle` kwarg (D:bin3D.py:114-115; tools.py:136 defaults --shuffle to True for training): the ordered candidate list
         is permuted before the feasibility tests and the leaf cap, by a keyed counter-based permutation (include/pct_b200.h, pct_config::shuffle)."""
         if not torch.cuda.is_available():
-            raise PctError("pct_b200 needs a CUDA device (sm_100a kernels; there is no CPU fallback)")
+            raise PctError("pct_b200 needs a CUDA device (sm_90a kernels; there is no CPU fallback)")
         self.L = _lib.lib()
         self.n_envs = int(n_envs)
         self.device = torch.device("cuda", device)

@@ -38,7 +38,7 @@ int continuous_query(pct_env_batch *h, int env, const double q[5], double densit
 
 extern "C" {
 
-const char *pct_version(void) { return "pct_b200 0.1 (sm_100a)"; }
+const char *pct_version(void) { return "pct_b200 0.1 (sm_90a)"; }
 
 const char *pct_last_error(pct_handle h) { return h ? h->err.c_str() : g_create_err.c_str(); }
 
@@ -52,8 +52,8 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
     if (device < 0 || device >= ndev) { g_create_err = "pct_create: bad device index"; return PCT_ERR_INVALID; }
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
-    if (prop.major != 10) {
-        g_create_err = std::string("pct_create: device '") + prop.name + "' is not sm_100 (kernels are built for sm_100a only)";
+    if (prop.major != 9 || prop.minor != 0) {
+        g_create_err = std::string("pct_create: device '") + prop.name + "' is not sm_90 (kernels are built for sm_90a only)";
         return PCT_ERR_NO_DEVICE;
     }
     if (cfg->setting < 1 || cfg->setting > 3) { g_create_err = "pct_create: setting must be 1, 2 or 3"; return PCT_ERR_INVALID; }
@@ -389,8 +389,8 @@ int pct_step_host(pct_handle h, const void *h_actions, int32_t action_f64, const
             const size_t n = (size_t)h->n_envs;
             // reward / done are write-only for the kernels too: when their buffers are pinned the apply kernel writes them straight into the mapped
             // host buffers (posted PCIe writes), saving two of the four staging copies.  Actions / leaf indices (READ by the apply kernel) and info
-            // (read-modify-write by the emit kernel) keep their staged copies: measured (round 2, call 14), device-side READS of mapped host memory
-            // put a PCIe round trip on every env's critical path — pct_step_host went from 426 to 661 us per step with everything mapped.
+            // (read-modify-write by the emit kernel) keep their staged copies: device-side READS of mapped host memory
+            // put a PCIe round trip on every env's critical path, and pct_step_host was measured markedly slower with everything mapped.
             auto alias = [](const void *hp) -> void * {
                 void *d = nullptr;
                 if (hp && cudaHostGetDevicePointer(&d, const_cast<void *>(hp), 0) == cudaSuccess && d) return d;

@@ -1,5 +1,5 @@
 // Shared device helpers: counter-based RNG, CPython tuple-hash / set-probe emulation, TMA (1-D bulk copy)
-// and mbarrier wrappers for sm_100a.
+// and mbarrier wrappers for sm_90a.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Continuous PCT environment (pct_envs/PctContinuous0 in the reference, "C:" below): batched reset / step for sm_100a.
+// Continuous PCT environment (pct_envs/PctContinuous0 in the reference, "C:" below): batched reset / step for sm_90a.
 //
 // Same three-kernel pipeline as the discrete domain (apply / candidates / feasibility+emit) and the same stability
 // routine (pct_stability.cuh) instantiated with a float64 geometry policy that carries the reference's 1e-6
@@ -220,12 +220,12 @@ __device__ __noinline__ int genems_warp_c(CEnv *ev, const int n0, const double l
     const int n = off < CE_TMP ? off : CE_TMP;
     __syncwarp();
     // EliminateInscribedEMS (C:space.py:505-528): the O(n^2) containment test read every candidate container b from the env record in global memory
-    // (ncu r2, profiles/r2_cont_head.txt: 30 % of this kernel's stall samples on that line); the intermediate list is staged in shared memory first
+    // (the line with the most stall samples in a profile of this kernel); the intermediate list is staged in shared memory first
     // (lists longer than CE_STAGE entries — not seen on the BASELINE streams — keep reading the record).
     const bool staged = n <= CE_STAGE;
     // Every EMS coordinate is a 6-decimal value (the container's corners or an np.around(.., 6) result), so v -> rint(v * 1e6) is an order-preserving
     // bijection onto integers; for bins up to 1.048575 they fit 20 bits and the six comparisons of a containment test become two 64-bit subtractions on
-    // packed fields with guard bits (the discrete kernel's trick; ncu r2: this loop was 21 % of the kernel's instructions).  Any coordinate that is not
+    // packed fields with guard bits (the discrete kernel's trick).  Any coordinate that is not
     // exactly such a value (checked per entry) sends the whole list through the float64 comparisons.
     constexpr uint64_t GUARD = (1ull << 20) | (1ull << 41) | (1ull << 62);
     uint64_t *pk = (uint64_t *)&stage[0][0];
@@ -441,8 +441,8 @@ __global__ void __launch_bounds__(64) pctc_apply_kernel(const CParams p) {
 // Table slots are 32 bits: candidate code | 16-bit tag (the top bits of the tuple hash — CPython compares the stored hash before the keys, setobject.c).
 // A probe rejects a non-matching slot on the tag alone; the exact 6-double comparison (tuples rebuilt from the two codes) runs only on a tag match,
 // i.e. practically only for true duplicates.  Round 1 rebuilt and compared the tuple of EVERY probed slot and broadcast the six doubles of every
-// inserted key through shuffles (ncu r2, profiles/r2_cont_head.txt: 25 % of this kernel in _Py_HashDouble's frexp loop — now an integer rotation,
-// pct_pyhash.cuh —, 15 % in shuffles).
+// inserted key through shuffles (a large share of this kernel's instructions went to _Py_HashDouble's frexp loop — now an integer rotation,
+// pct_pyhash.cuh — and to shuffles).
 __device__ __forceinline__ bool cand_equal(uint16_t a, uint16_t b, const double (*ems)[6], const double nb[3]) {
     double u[6], v[6];
     cand_tuple(a, ems, nb, u);
@@ -482,7 +482,7 @@ __global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
         uint16_t code = 0;
         // The four corners of one (EMS, orientation) are four adjacent lanes and their 6-tuples draw on ten distinct coordinates (x: m0, m0 + sx, m3 - sx,
         // m3; y alike; z: m2, m2 + sz): every lane hashes two or three of them (_Py_HashDouble, the expensive part) and the group exchanges the results,
-        // instead of six hashes per lane (ncu r2: 17 % of this kernel's instructions).  Same expressions as cand_tuple, so the same bits.
+        // instead of six hashes per lane.  Same expressions as cand_tuple, so the same bits.
         uint64_t h0 = 0, h1 = 0, h2 = 0;
         const int q = r & 3;
         if (r < raw) {

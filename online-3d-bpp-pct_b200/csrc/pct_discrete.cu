@@ -1,4 +1,4 @@
-// Discrete PCT environment: batched reset / step kernels for sm_100a.
+// Discrete PCT environment: batched reset / step kernels for sm_90a.
 //
 // One warp owns one environment for the whole step:
 //   TMA bulk load of the env's packed record (header + placed boxes + EMS list) HBM -> shared memory
@@ -40,8 +40,8 @@ namespace pct {
 // The CPython-set emulation walks table sizes 8 -> 32 -> 128 -> 512 -> 2048, alternating between two buffers:
 // A holds the 8 / 128 / 2048 stages, B the 32 / 512 stages.  BIGSM = true keeps the 2048 stage in shared memory
 // (setting 2: 6 orientations, hundreds of candidates per step); BIGSM = false (settings 1/3: <= 306 candidates in
-// practice) keeps A at 128 slots and spills the rare 2048 stage to the env's cold record in HBM, which lets 28
-// warps (= 4096 envs / 148 SMs) be resident per SM.
+// practice) keeps A at 128 slots and spills the rare 2048 stage to the env's cold record in HBM, which keeps a warp's
+// share of shared memory at ~5 KB: 32 warps fit in one SM (4096 envs on 132 SMs need ceil(4096 / 132) = 32).
 template <typename SlotT, bool BIGSM>
 struct Lay {
     static constexpr int A_SLOTS = BIGSM ? TAB_A : 128;
@@ -167,7 +167,7 @@ __device__ __noinline__ int genems_warp(int16_t (*ems)[6], const int n0, int16_t
     const int n = off < EMS_TMP_MAX ? off : EMS_TMP_MAX;  // intermediate list (survivors + children), before the inscribed-EMS purge
     __syncwarp();
     // EliminateInscribedEMS: drop i if some j != i contains it (non-strict; identical twins delete each other).
-    // The O(n^2) containment test was 28 % of the apply kernel's warp instructions (ncu r2, profiles/r2_k1_head_source.txt): six 16-bit loads and
+    // The O(n^2) containment test was a large share of the apply kernel's warp instructions: six 16-bit loads and
     // six compares per pair.  Coordinates are <= 255 (pct_create), so an EMS packs into two words of three 9-bit fields — lows as they are, highs
     // as 255 - v, which turns all six tests into "field of a >= field of b" — and with a guard bit per field one subtraction tests three fields:
     // ((a | G) - b) keeps the guard of a field iff a_f >= b_f (fields are >= 1 after the OR, so no borrow crosses a field).
@@ -674,7 +674,7 @@ __device__ __noinline__ void write_obs_delta(const DParams &p, int e, const DEnv
 
 // ======================================================================================================
 // The step is a pipeline of three kernels (plus the optional synthetic-policy kernel).  A monolithic
-// one-warp-per-env kernel was measured first (profiles/r1_monolithic_*.txt): it was instruction-fetch bound
+// one-warp-per-env kernel was measured first: it was instruction-fetch bound
 // (each warp streamed ~80 KB of SASS once per step, warps of an SM sat in different phases) and its duration
 // was the latency of the slowest env.  Splitting by phase keeps every kernel's code small and hot in the
 // instruction cache and lets the heavy phase run one THREAD per candidate leaf.
@@ -1219,9 +1219,9 @@ __global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(co
 }
 
 // ---- K3 (round 2): pooled stability walks + emit ---------------------------------------------------------------------
-// ncu of the kernel above at round 1's HEAD (profiles/r2_k3_head_*.txt) and of a warp-per-env variant (profiles/r2_k3_warp_per_env.txt):
+// Profiles of the kernel above (round 1) and of a warp-per-env variant:
 // the launch lasts 2x the SMs' mean active time — it ends when the env with the most and deepest stability walks ends (a serial chain
-// inside one block) —, 60 % of the warp instructions sit in the walk at 2-5 active lanes, every candidate scans the boxes twice, and capping
+// inside one block) —, most of the warp instructions sit in the walk at 2-5 active lanes, every candidate scans the boxes twice, and capping
 // registers for occupancy only trades stalls for spills.  Round 2 cuts the work by KIND instead of by env:
 //   classify  (end of K2, warp per env, integer only) bounds + ONE pass over the boxes for resting height, supports and the exact
 //             quick reject (rest_height_supports) -> infeasible / feasible / needs a stability walk; feasibility bits per 32-candidate
@@ -1331,8 +1331,8 @@ __global__ void __launch_bounds__(32 * LIGHT_WARPS, LIGHT_MINB) pct_walk_light_k
 
 // walk, stage 2: the continuations — every lane starts with the heavy visit its walk stopped at, then runs the general light / heavy state
 // machine to the end of the walk.  Only `p.walk_lanes` lanes of a warp carry a walk (default 16; 4 for the walks resting at >= 0.6 H): there are few
-// continuations (3 per env) and each is a long serial chain; a full warp of them (ncu r2, profiles/r2_walk_two_stage_32lanes.txt: 400 warps on 592
-// schedulers, 20 k instructions per warp, 116 us) leaves too few warps, 4-8 per warp multiply the warp instructions (measured sweep: DESIGN.md 5d).
+// continuations (3 per env) and each is a long serial chain; a full warp of them leaves
+// fewer warps than the SMs have schedulers, 4-8 per warp multiply the warp instructions (measured sweep).
 __global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_kernel(const DParams p) {
     const int lane = threadIdx.x & 31;
     const int cap = p.n_envs * WALK_CONT_PER_ENV;
@@ -1366,8 +1366,8 @@ __global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_kernel(co
 // its first subtree and publishes the other k - 1 as new pieces; protocol: pct_walkq.cuh).  A walk's verdict is the AND over its pieces:
 // walk_pend[item] counts them, the piece that brings it to zero sets the feasibility bit (unless one failed) and releases the env's n_pending.
 // The critical chain of a step's longest walk becomes its longest root-to-floor PATH instead of the sum over its visits (host statistics,
-// scratch/stats_paths.py: 51 -> 34 visit units at the 99.99 % quantile) — and the stage does not get faster (B200, 4096 envs: walk + emit group 0.180 ms
-// against 0.171 ms, whatever the number of helper warps, blocks per SM or pieces per warp): the continuation stage is bound by the issue rate of a few
+// scratch/stats_paths.py: 51 -> 34 visit units at the 99.99 % quantile) — and the stage did not get faster in
+// measurements, whatever the number of helper warps, blocks per SM or pieces per warp: the continuation stage is bound by the issue rate of a few
 // hundred divergent, latency-bound warps (warp instructions = thread instructions / 4.8 lanes, ~10 cycles each), not by its longest walk.  Kept as an
 // opt-in because it is the measured answer to "would independent subtrees on separate lanes help?" and is parity-tested (tests/test_gpu_walk_fork.py).
 struct PieceFork {

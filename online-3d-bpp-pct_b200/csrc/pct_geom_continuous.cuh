@@ -7,8 +7,8 @@
 
 namespace pct {
 
-// np.around(v, 6) = rint(v * 1e6) / 1e6.  The correctly rounded IEEE division is a ~30-instruction subroutine on the GPU and was 18 % of the continuous
-// feasibility kernel's warp instructions (ncu r2, profiles/r2_cont_head_source.txt).  For the constant divisor 1e6 the quotient of an integer-valued a follows
+// np.around(v, 6) = rint(v * 1e6) / 1e6.  The correctly rounded IEEE division is a ~30-instruction subroutine on the GPU and was a large share of the
+// continuous feasibility kernel's warp instructions.  For the constant divisor 1e6 the quotient of an integer-valued a follows
 // from the correctly rounded reciprocal y = 1e-6 by one FMA correction (Markstein): q0 = a * y, r = fma(-q0, 1e6, a) (exact), q = fma(r, y, q0).
 // scratch/around6_exhaustive.c checks q == a / 1e6 for EVERY integer |a| <= 2.2e9 (|v| <= 2200 at 6 decimals): 0 mismatches (q0 alone: 30 %); beyond
 // that range the exact division runs.  tests/test_oracle_units.py::test_fast_around6_equals_the_division samples it through the host build.

@@ -24,8 +24,8 @@ struct pct_env_batch {
     int32_t *d_ready = nullptr;   // [2 * n_envs] per-env hand-over flags of the overlapped launch mode
     int32_t epoch = 0;
     bool overlap = true;          // PCT_B200_OVERLAP=0: plain back-to-back kernels
-    bool overlap_cont = false;    // continuous domain: measured slower overlapped (5.35 M -> 3.97 M env-steps/s), off unless PCT_B200_OVERLAP_CONT=1
-    // delta observation writes (default ON since round 2: +3 % device path, and with zero-copy 5.2 -> 9.1 M env-steps/s through pct_step_host;
+    bool overlap_cont = false;    // continuous domain: measured slower overlapped, off unless PCT_B200_OVERLAP_CONT=1
+    // delta observation writes (default ON since round 2: faster on the device path, and much faster through pct_step_host with zero-copy;
     // PCT_B200_OBS_DELTA=0 disables): the feasibility kernel writes only the rows that can differ from what the SAME caller buffer already holds
     // (DEnvAux::obs_prev = per env the internal / leaf rows of the tracked buffer that may be non-zero).  Contract (include/pct_b200.h): a caller
     // that hands the same observation pointer to consecutive calls must not have modified the buffer in between.
@@ -40,7 +40,7 @@ struct pct_env_batch {
     const void *tracked_obs = nullptr;
     bool fill_pending = false;
     bool host_zero_copy = true;   // pct_step_host: kernels write the observation straight into the pinned (mapped) host buffer; PCT_B200_HOST_ZEROCOPY=0: staged copies
-    bool cont_pre = true;         // continuous feas_emit: resting heights from pre-rounded rectangles (exact, +2 %; PCT_B200_CONT_PRE=0 disables)
+    bool cont_pre = true;         // continuous feas_emit: resting heights from pre-rounded rectangles (exact; PCT_B200_CONT_PRE=0 disables)
     int32_t *d_hstate = nullptr;  // (n_envs, 4) LSAH footprint state (pct_heuristic_actions)
     double *d_hstate_c = nullptr; // same for the continuous domain (pct_heuristic_actions_f64)
     double *d_query_c = nullptr;  // 2 doubles: result of pct_query_placement_f64
@@ -61,9 +61,9 @@ struct pct_env_batch {
     int32_t *d_cont_ctr = nullptr;
     size_t contq_env_bytes = 0;        // bytes of d_contq per env (WalkCont pool / WalkPiece queue)
     int32_t *d_piece_ready = nullptr, *d_walk_pend = nullptr;  // fork-join walks: per-slot publication flags, per-walk piece counters
-    bool walk_fork = false;            // PCT_B200_WALK=fork: fork-join continuation kernel (pct_walkq.cuh) instead of the sequential one — measured equal-to-slower (DESIGN.md 5d), kept as an opt-in
+    bool walk_fork = false;            // PCT_B200_WALK=fork: fork-join continuation kernel (pct_walkq.cuh) instead of the sequential one — measured equal-to-slower (DESIGN.md section 5), kept as an opt-in
     int walk_blocks = 6;               // its blocks per SM (PCT_B200_WALK_BLOCKS)
-    int walk_keep = 296;               // its warps that stay as helpers for forked pieces (PCT_B200_WALK_KEEP)
+    int walk_keep = 264;               // its warps that stay as helpers for forked pieces: two per SM of the H100 (PCT_B200_WALK_KEEP)
     int walk_lanes_tall = 4;           // ... of the tall walks (resting height >= 0.6 H: the longest chains), PCT_B200_WALK_LANES_TALL
     int walk_lanes = 16;               // continuations per warp of pct_walk_kernel (PCT_B200_WALK_LANES; few long serial chains: more warps beat fuller warps)
     bool lpt = false;

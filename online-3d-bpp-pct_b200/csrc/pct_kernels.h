@@ -30,7 +30,7 @@ constexpr int EDGE_MAX = 255;    // load edges per env; positions are uint8, 255
 constexpr int EDGE_NIL = 255;
 // Staging areas of the apply kernel.  Small on purpose: its descent runs on ONE lane per warp, so every hot word of that lane's local-memory stack
 // costs a whole 128-byte L1 line; 64 loads + 96 vertices per warp put the kernel at the 164 KB shared-memory carve-out (92 KB of L1), 16 + 32 at
-// the 132 KB one (124 KB of L1): apply kernel 0.1126 -> 0.1075 ms (B200, 4096 envs; r2_c25).  Entries beyond the staged ones are read from L1 / L2.
+// the 132 KB one (124 KB of L1), which leaves that stack more L1.  Entries beyond the staged ones are read from L1 / L2.
 #ifndef PCT_EDGE_STAGE
 #define PCT_EDGE_STAGE 16
 #endif

@@ -7,7 +7,7 @@
 //   Space.scale_down                                    D:space.py:341-345
 //   np.linalg.lstsq for >=3 supports                    D:space.py:137-152, 234-250
 //
-// B200 restatement (not a translation):
+// CUDA restatement (not a translation):
 //   * no objects, no recursion: an explicit DFS over the support DAG with a small per-lane frame stack;
 //   * supports, contact rectangles, hulls are recomputed from the packed box records in shared memory
 //     instead of being stored per box;
@@ -714,7 +714,7 @@ static __device__ __noinline__ int stability_check(const G &g, const typename G:
 // stab_virtual: the read-only feasibility check (calculated_impact_virtual, D:space.py:166-267) for a WARP of placements,
 // one lane per placement, restructured for SIMT convergence (round 2).
 //
-// ncu of round 1's thread-per-candidate kernel (profiles/r2_k3_head_source.txt): the DFS of stability_check<false> holds 60 % of
+// In round 1's thread-per-candidate kernel the DFS of stability_check<false> held most of
 // the kernel's warp instructions at 2-5 active lanes — every lane walks its own support DAG, and a visit is either LIGHT (no or
 // one support: a rectangle test in registers) or HEAVY (>= 2 supports: hull / stored polygon, load split, frame push), 10x the
 // instructions; with both kinds present in nearly every round a warp pays light + heavy per round.  Here the walk is a per-lane state machine with

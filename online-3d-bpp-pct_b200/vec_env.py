@@ -86,7 +86,7 @@ class PctVecEnv(object):
                  leaf_node_holder=50, continuous=False, device=0, seed=0, env_id_base=0, sample_from_distribution=False,
                  sample_left_bound=None, sample_right_bound=None, item_stream=None, LNES="EMS", shuffle=False, copy_obs=True,
                  raise_on_flags=True, **_ignored):
-        """copy_obs: return a fresh observation tensor every step like VecPyTorch does (a 19 MB device copy at 4096 envs, ~6 us); False hands
+        """copy_obs: return a fresh observation tensor every step like VecPyTorch does (a 19 MB device-to-device copy at 4096 envs); False hands
         out the library-owned buffer that the next step rewrites in place (zero-copy; the caller must not modify it: delta observation rows).
         shuffle: the reference's kwarg (np.random.shuffle of the candidate list, D:bin3D.py:114-115) as a keyed device-side permutation (PctBatch).
         raise_on_flags: a capacity / hand-over flag in any env's step record (pct_step_info.flags: overflowed EMS / candidate / edge / support

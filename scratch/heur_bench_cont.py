@@ -1,5 +1,5 @@
 import sys, time, torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, __import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))))
 import pct_b200
 items = [(round(0.1 * i, 1), round(0.1 * j, 1), round(0.1 * k, 1)) for i in range(1, 6) for j in range(1, 6) for k in range(1, 6)]
 for name, setting, n in (("LSAH", 2, 4096), ("OnlineBPH", 2, 4096), ("BR", 2, 4096), ("LSAH", 1, 4096), ("OnlineBPH", 1, 4096), ("BR", 1, 4096)):

@@ -1,5 +1,5 @@
 import sys, time
-sys.path.insert(0, '/root/repo/oracle')
+sys.path.insert(0, __import__('os').path.join(__import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))), 'oracle'))
 import numpy as np
 import ref_shim, pct_oracle
 from pct_oracle import OracleDiscrete, policy_pick, rnd_u64

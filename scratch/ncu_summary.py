@@ -1,6 +1,6 @@
-"""ncu_summary.py REPORT.ncu-rep [N_LINES] — text summary of an `ncu --set full --import-source on` capture for profiles/: per launch the duration, DRAM
+"""ncu_summary.py REPORT.ncu-rep [N_LINES] — text summary of an `ncu --set full --import-source on` capture: per launch the duration, DRAM
 bytes, registers, occupancy limits, instruction counts, lanes per instruction, local / shared / global memory instructions, IPC, stall reasons, and the
-top source lines by stall samples (needs -lineinfo).  Also prints one JSON line per launch with the DRAM traffic (for profiles/traffic.json)."""
+top source lines by stall samples (needs -lineinfo).  Also prints one JSON line per launch with the DRAM traffic."""
 import csv
 import io
 import json

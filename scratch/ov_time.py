@@ -1,5 +1,5 @@
 import sys, time, torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, __import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))))
 import pct_b200
 n = int(sys.argv[1]); setting = int(sys.argv[2])
 items = [(i, j, k) for i in range(1, 6) for j in range(1, 6) for k in range(1, 6)]

@@ -1,5 +1,5 @@
 import sys, time, torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, __import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))))
 for mb in (4.83, 19.3, 38.6, 256):
     nb = int(mb * 1e6)
     d = torch.empty(nb, dtype=torch.uint8, device='cuda'); h = torch.empty(nb, dtype=torch.uint8, pin_memory=True)

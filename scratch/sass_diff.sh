@@ -7,7 +7,7 @@ set -e
 REF=${1:-HEAD}; MAP=${2:-}
 ROOT=$(cd "$(dirname "$0")/.." && pwd); T=$(mktemp -d)
 git -C "$ROOT" archive "$REF" online-3d-bpp-pct_b200/csrc include | tar -x -C "$T"
-FLAGS="-O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC -I$T/include -I$T/online-3d-bpp-pct_b200/csrc -gencode arch=compute_100a,code=sm_100a"
+FLAGS="-O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC -I$T/include -I$T/online-3d-bpp-pct_b200/csrc -gencode arch=compute_90a,code=sm_90a"
 norm() { grep -E "^\s+/\*[0-9a-f]{4,6}\*/" | sed 's#/\*[0-9a-f]*\*/##'; }
 for u in pct_discrete pct_continuous; do
   nvcc $FLAGS -c "$T/online-3d-bpp-pct_b200/csrc/$u.cu" -o "$T/$u.o"

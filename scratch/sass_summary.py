@@ -1,5 +1,5 @@
-"""python scratch/sass_summary.py [lib.so] > profiles/r2_sass_opcodes.txt — per kernel of libpct_b200.so: SASS instruction count and the opcodes that
-prove the Blackwell-native paths (B200_PROFILING.md): UBLKCP (1-D TMA bulk copy, cp.async.bulk), SYNCS (mbarrier), PREEXIT (griddepcontrol.launch_dependents,
+"""python scratch/sass_summary.py [lib.so] — per kernel of libpct_b200.so: SASS instruction count and the opcodes that
+show the Hopper-native paths: UBLKCP (1-D TMA bulk copy, cp.async.bulk), SYNCS (mbarrier), PREEXIT (griddepcontrol.launch_dependents,
 programmatic dependent launch), plus the FP64 / vote / shuffle / atomic / local-memory mix.  No GPU needed (cuobjdump -sass)."""
 import collections, re, subprocess, sys
 lib = sys.argv[1] if len(sys.argv) > 1 else "online-3d-bpp-pct_b200/libpct_b200.so"

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a GPU machine)")
     config.addinivalue_line("markers", "reference: needs the read-only reference checkout at /root/reference")
 
 

@@ -105,62 +105,52 @@ def test_facade_dataset_handling_continuous(fake, tmp_path):
     assert np.allclose([r[0] for r in rec], ratio[:5], rtol=0, atol=1e-12)
 
 
-# ---- the vector surface against the reference's OWN wrappers (build container only) ---------------------------------------------
+# ---- the vector surface against the reference's OWN wrappers ----------------------------------------------------------------------
+import json  # noqa: E402
+import sys  # noqa: E402
+
 import ref_shim  # noqa: E402
 
+sys.path.insert(0, G)
+import make_reference_surface as RS  # noqa: E402
+from make_reference_lockstep import obs_digest  # noqa: E402
 
-@pytest.mark.reference
-@pytest.mark.skipif(not ref_shim.reference_available(), reason="reference not mounted")
+SURFACE = np.load(os.path.join(G, "reference_surface.npz"))
+
+
 @pytest.mark.parametrize("setting", [1, 2])
-def test_vec_env_equals_reference_shmem_vecpytorch_monitor(fake, setting, tmp_path, monkeypatch):
+def test_vec_env_equals_reference_shmem_vecpytorch_monitor(fake, setting, monkeypatch):
     """VecPyTorch(ShmemVecEnv([Monitor(PackingDiscrete)] * N, context='fork')) of the unmodified reference (envs.py:75-116,159-182,
-    wrapper/shmem_vec_env.py, wrapper/monitor.py) next to PctVecEnv: observation tensors, reward shape / values, done array, info
-    dicts (terminal ones with Monitor's 'episode' entry, the auto-reset observation) over 70 vector steps."""
-    from harness import make_stream, policy_pick
+    wrapper/shmem_vec_env.py, wrapper/monitor.py), recorded by tests/golden/make_reference_surface.py, next to PctVecEnv: observation
+    tensors, reward shape / values, done array, info dicts (terminal ones with Monitor's 'episode' entry, the auto-reset observation)
+    over 70 vector steps."""
     monkeypatch.setattr(importlib.import_module("pct_b200.vec_env"), "PctBatch", FakeBatch)
     import pct_b200
-    D, _ = ref_shim.load_reference()
-    renvs = importlib.import_module("envs")
-    ShmemVecEnv = importlib.import_module("wrapper.shmem_vec_env").ShmemVecEnv
-    Monitor = importlib.import_module("wrapper.monitor").Monitor
-    n, seed = 5, 50 + setting
-    streams = np.stack([make_stream(seed, e, 300, setting) for e in range(n)])
-
-    def thunk(rank):
-        def _t():
-            env = D.PackingDiscrete(setting=setting, container_size=[10, 10, 10], item_set=ITEM_SET, internal_node_holder=80, leaf_node_holder=50,
-                                    shuffle=False, LNES="EMS")
-            env.box_creator = ref_shim.make_stream_creator(D, [tuple(int(v) for v in r[:3]) for r in streams[rank]])
-            env.test = True
-            return Monitor(env, os.path.join(str(tmp_path), str(rank)), allow_early_resets=True)
-        return _t
-
-    probe = D.PackingDiscrete(setting=setting, container_size=[10, 10, 10], item_set=ITEM_SET)
-    ref = renvs.VecPyTorch(ShmemVecEnv([thunk(r) for r in range(n)], [probe.observation_space, probe.action_space], context="fork"), "cpu")
-    ours = pct_b200.PctVecEnv(n, setting, item_set=ITEM_SET, item_stream=streams)
+    ref = {k: SURFACE["vec_s%d_%s" % (setting, k)] for k in ("obs", "reward", "done", "info")}
+    dt = json.loads(str(SURFACE["vec_s%d_dtypes" % setting]))
+    n = RS.VEC_ENVS
+    ours = pct_b200.PctVecEnv(n, setting, item_set=ITEM_SET, item_stream=RS.vec_streams(setting))
     try:
-        o_ref, o = ref.reset(), ours.reset()
-        assert o_ref.dtype == o.dtype == torch.float32 and tuple(o.shape) == tuple(o_ref.shape) == (n, 1179)
+        o = ours.reset()
+        assert dt["obs"] == str(o.dtype) == "torch.float32" and list(o.shape) == dt["obs_shape"] == [n, 1179]
         dones = 0
-        for t in range(70):
-            assert torch.equal(o_ref, o), "observations before step %d" % t
-            rows = np.stack([policy_pick(o_ref[e].numpy().astype(np.float64), 80, 50, seed, e, t)[1] for e in range(n)]).astype(np.float32)
-            o_ref, r_ref, d_ref, i_ref = ref.step(rows)  # float32 numpy leaf rows, as train_tools.py:66-67 passes them
-            o, r, d, i = ours.step(rows)
-            assert tuple(r.shape) == tuple(r_ref.shape) == (n, 1) and r.dtype == r_ref.dtype and torch.equal(r, r_ref)
-            assert d.dtype == d_ref.dtype == np.bool_ and np.array_equal(d, d_ref)
-            for e in range(n):
-                assert i[e]["counter"] == i_ref[e]["counter"]
-                if d_ref[e]:
+        for t in range(RS.VEC_STEPS):
+            assert obs_digest(o.numpy()) == ref["obs"][t], "observations before step %d" % t
+            o, r, d, i = ours.step(RS.vec_rows(o.numpy(), setting, t))
+            assert list(r.shape) == dt["reward_shape"] == [n, 1] and str(r.dtype) == dt["reward"] and np.array_equal(r.numpy()[:, 0], ref["reward"][t])
+            assert d.dtype == np.bool_ and str(d.dtype) == dt["done"] and np.array_equal(d, ref["done"][t])
+            for e, want in enumerate(json.loads(str(ref["info"][t]))):
+                assert i[e]["counter"] == want["counter"] and sorted(i[e]) == want["keys"]
+                if ref["done"][t][e]:
                     dones += 1
-                    assert set(i_ref[e]) == set(i[e]) == {"counter", "ratio", "reward", "episode"}
-                    assert abs(i[e]["ratio"] - i_ref[e]["ratio"]) < 1e-6 and abs(i[e]["reward"] - i_ref[e]["reward"]) < 1e-5
-                    assert i[e]["episode"]["l"] == i_ref[e]["episode"]["l"] and abs(i[e]["episode"]["r"] - i_ref[e]["episode"]["r"]) < 1e-4
+                    assert want["keys"] == ["counter", "episode", "ratio", "reward"]
+                    assert abs(i[e]["ratio"] - want["ratio"]) < 1e-6 and abs(i[e]["reward"] - want["reward"]) < 1e-5
+                    assert i[e]["episode"]["l"] == want["l"] and abs(i[e]["episode"]["r"] - want["r"]) < 1e-4
                 else:
-                    assert set(i[e]) == set(i_ref[e]) == {"counter"}
+                    assert want["keys"] == ["counter"]
+        assert obs_digest(o.numpy()) == ref["obs"][RS.VEC_STEPS]
         assert dones >= 8
     finally:
-        ref.close()
         ours.close()
 
 
@@ -231,17 +221,16 @@ def test_unmodified_heuristic_functions_run_on_the_continuous_facade(fake, name,
     assert env.log[:3] == packed[:3]
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not ref_shim.reference_available(), reason="reference not mounted")
-@pytest.mark.parametrize("argv,continuous", [(["--setting", "1", "--num-processes", "6", "--seed", "9"], False),
-                                              (["--setting", "2", "--continuous", "--sample-from-distribution", "--num-processes", "4"], True)])
+@pytest.mark.parametrize("argv,continuous", [(RS.ARGVS["discrete"], False), (RS.ARGVS["continuous"], True)])
 def test_make_vec_envs_takes_the_reference_args(fake, argv, continuous, monkeypatch):
-    """envs.make_vec_envs(args, log_dir, allow_early_resets) (envs.py:75-116) with the namespace tools.get_args() builds"""
+    """envs.make_vec_envs(args, log_dir, allow_early_resets) (envs.py:75-116) with the namespace tools.get_args() builds from `argv`
+    (recorded by tests/golden/make_reference_surface.py)"""
+    import argparse
     import pct_b200
-    from pct_oracle import OracleBatch
-    compat = importlib.import_module("pct_b200.compat")
     monkeypatch.setattr(importlib.import_module("pct_b200.vec_env"), "PctBatch", FakeBatch)
-    args = compat.reference_args(ref_shim.REFERENCE_ROOT, argv)
+    ns = json.loads(str(SURFACE["args"]))["continuous" if continuous else "discrete"]
+    ns["item_size_set"] = [tuple(s) for s in ns["item_size_set"]]  # givenData.py: a list of tuples (JSON stores lists)
+    args = argparse.Namespace(**ns)
     if continuous:
         args.container_size = [1, 1, 1]  # givenData.py:5 (the commented alternative)
         args.sample_left_bound, args.sample_right_bound = 0.1, 0.5

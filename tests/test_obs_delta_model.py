@@ -2,7 +2,7 @@
 restated in numpy and run over oracle trajectories with episode ends and resets: a buffer that only ever receives the rows the rule
 selects must equal the full observation after every step — including when the buffer is swapped for one full of garbage (the host
 then resets the row counts to "all", begin_obs / pct_fill_prev_kernel in csrc/pct_api.cu).  This checks the algorithm and its
-invariant (rows at or above the stored counts are all-zero), not the CUDA code; tests/test_zzz_gpu_obs_delta.py does that on a B200."""
+invariant (rows at or above the stored counts are all-zero), not the CUDA code; tests/test_zzz_gpu_obs_delta.py does that on an H100."""
 import numpy as np
 import pytest
 

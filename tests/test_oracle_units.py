@@ -74,31 +74,22 @@ def test_lstsq_rank_deficient_minimum_norm():
     assert np.allclose(x, want, rtol=1e-6, atol=1e-9)
 
 
-@pytest.mark.reference
 def test_hull_and_pip_match_reference_module():
-    import ref_shim
-    if not ref_shim.reference_available():
-        pytest.skip("reference not mounted")
-    D, _ = ref_shim.load_reference()
-    from pct_envs.PctDiscrete0.convex_hull import ConvexHull, point_in_polygen
-    from pct_envs.PctDiscrete0.space import Space
-    sp = Space(10, 10, 10, 1, 80)
-    rng = np.random.RandomState(3)
-    for trial in range(600):
-        k = rng.choice([1, 1, 2, 2, 3, 4, 6])
-        pts = []
-        for _ in range(k):
-            x1, y1 = rng.randint(0, 8, 2); x2, y2 = x1 + rng.randint(1, 4), y1 + rng.randint(1, 4)
-            pts += [[x1, y1], [x1, y2], [x2, y1], [x2, y2]]
-        want = np.array(sp.scale_down(ConvexHull([list(p) for p in pts])))
+    """the oracle's shrunk hull and point-in-polygon test against the reference's ConvexHull / scale_down / point_in_polygen
+    (D:convex_hull.py, D:space.py), whose results tests/golden/make_reference_lockstep.py recorded"""
+    import os
+    import sys
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+    from make_reference_lockstep import hull_trials, obs_digest
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_lockstep.npz"))
+    for trial, (pts, qs) in enumerate(hull_trials()):
         p = np.array(pts, dtype=np.float64)
         out = np.zeros((2 * len(pts), 2))
         m = L.pcto_hull_shrunk(p.ctypes.data_as(C.POINTER(C.c_double)), len(pts), out.ctypes.data_as(C.POINTER(C.c_double)))
-        assert m == len(want) and np.array_equal(out[:m], want), trial
-        for _ in range(6):
-            q = np.array([rng.randint(0, 20) / 2.0, rng.randint(0, 20) / 2.0]) if rng.rand() < 0.5 else rng.uniform(0, 10, 2)
-            got = L.pcto_pip(q[0], q[1], np.ascontiguousarray(want).ctypes.data_as(C.POINTER(C.c_double)), m)
-            assert bool(got) == bool(point_in_polygen(q, want.tolist()))
+        assert m == g["hull_count"][trial] and obs_digest(out[:m]) == g["hull_digest"][trial], trial
+        hull = np.ascontiguousarray(out[:m])
+        for q, want in zip(qs, g["hull_pip"][trial]):
+            assert bool(L.pcto_pip(q[0], q[1], hull.ctypes.data_as(C.POINTER(C.c_double)), m)) == bool(want)
 
 
 def test_around6_commutes_with_min():

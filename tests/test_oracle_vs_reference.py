@@ -1,43 +1,54 @@
-"""CPU, build container only: live lock-step of the C oracle against the unmodified Python reference
-(every observation including terminal ones, reward, done, info).  Skipped where /root/reference is absent."""
+"""CPU: lock-step of the C oracle against the unmodified Python reference (every observation including terminal ones, reward, done,
+info), replayed from what the reference produced: tests/golden/reference_lockstep.npz, recorded by tests/golden/make_reference_lockstep.py."""
+import json
+import os
+import sys
+
 import numpy as np
 import pytest
 
-import ref_shim
 from harness import ITEM_SET, make_stream, policy_pick
 from pct_oracle import OracleDiscrete
 
-pytestmark = [pytest.mark.reference, pytest.mark.skipif(not ref_shim.reference_available(), reason="reference not mounted")]
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+from harness import CASES, CONT_CASES  # noqa: E402
+from make_reference_lockstep import CASE_STEPS, CONT_CASE_STEPS, LOCKSTEP_STEPS, TIE_ENV, TIE_SEED, TIE_STEPS, info_text, obs_digest  # noqa: E402
+
+G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_lockstep.npz"))
 
 
 @pytest.mark.parametrize("setting", [1, 2, 3])
 def test_lockstep_with_reference(setting):
-    D, _ = ref_shim.load_reference()
-    seed, env_id, steps = 900 + setting, 3, 260
-    stream = make_stream(seed, env_id, steps + 64, setting)
-    ref = D.PackingDiscrete(setting=setting, container_size=[10, 10, 10], item_set=ITEM_SET, internal_node_holder=80,
-                            leaf_node_holder=50, shuffle=False, LNES="EMS")
-    ref.box_creator = ref_shim.make_stream_creator(D, [tuple(r) if setting == 3 else tuple(int(v) for v in r[:3]) for r in stream])
-    ref.test = True
-    orc = OracleDiscrete(setting, stream=stream)
-    o1, o2 = ref.reset(), orc.reset()
+    ref = {k: G["lockstep_s%d_%s" % (setting, k)] for k in ("obs", "reward", "done", "info")}
+    seed, env_id = 900 + setting, 3
+    orc = OracleDiscrete(setting, stream=make_stream(seed, env_id, LOCKSTEP_STEPS + 64, setting))
+    o = orc.reset()
+    k = 0
+    for t in range(LOCKSTEP_STEPS):
+        assert obs_digest(o) == ref["obs"][k], t
+        _, row = policy_pick(o, 80, 50, seed, env_id, t)
+        o, r, d, i = orc.step(row)
+        k += 1
+        assert obs_digest(o) == ref["obs"][k], "observation after step %d (done=%s)" % (t, d)
+        assert (r, d) == (ref["reward"][t], ref["done"][t]) and json.loads(info_text(i)) == json.loads(str(ref["info"][t]))
+        if d:
+            o = orc.reset()
+            k += 1
+    assert k == len(ref["obs"]) - 1
+
+
+# ---- other configurations on fresh seeds (the committed full records of the same configurations are tests/golden/case_*.npz) ----
+def _lockstep_record(orc, c, seed, env_id, steps):
+    o = orc.reset()
+    obs, rew, done, counter, ratio = [obs_digest(o)], [], [], [], []
     for t in range(steps):
-        assert np.array_equal(o1, o2), t
-        _, row = policy_pick(o1, 80, 50, seed, env_id, t)
-        o1, r1, d1, i1 = ref.step(row)
-        o2, r2, d2, i2 = orc.step(row)
-        assert np.array_equal(o1, o2), "observation after step %d (done=%s)" % (t, d1)
-        assert (r1, d1) == (r2, d2) and i1 == i2
-        if d1:
-            o1, o2 = ref.reset(), orc.reset()
-
-
-# ---- other configurations, live (fresh seeds; the committed records of the same configurations are tests/golden/case_*.npz) ----
-import os  # noqa: E402
-import sys  # noqa: E402
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from harness import CASES, CONT_CASES  # noqa: E402
+        _, row = policy_pick(o, c["nb"], c["nl"], seed, env_id, t)
+        o, r, d, info = orc.step(row)
+        obs.append(obs_digest(o)); rew.append(r); done.append(d); counter.append(info["counter"]); ratio.append(info.get("ratio", -1.0))
+        if d:
+            o = orc.reset()
+            obs.append(obs_digest(o))
+    return dict(obs=np.array(obs), reward=np.array(rew), done=np.array(done), counter=np.array(counter), ratio=np.array(ratio))
 
 
 def _equal_records(a, b):
@@ -48,88 +59,43 @@ def _equal_records(a, b):
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_cases_lockstep_with_reference(name):
     """the recorder of tests/golden/make_golden_cases.py on the reference vs the same loop on the oracle, new seed"""
-    import make_golden_cases as M
     from harness import case_stream
-    D, _ = ref_shim.load_reference()
-    c = dict(CASES[name], steps=60)
-    ref = M.record_case(D, c, 8800, 4)
-
+    c = dict(CASES[name], steps=CASE_STEPS)
     orc = OracleDiscrete(c["setting"], container_size=c["container"], internal_node_holder=c["nb"], leaf_node_holder=c["nl"],
                          size_minimum=min(min(i) for i in c["items"]), stream=case_stream(c, 8800, 4, c["steps"] + 64), lnes=c["lnes"])
-    o = orc.reset()
-    obs, rew, done, counter, ratio = [o.copy()], [], [], [], []
-    for t in range(c["steps"]):
-        o, r, d, info = orc.step(ref["rows"][t])
-        obs.append(o.copy()); rew.append(r); done.append(d); counter.append(info["counter"]); ratio.append(info.get("ratio", -1.0))
-        if d:
-            o = orc.reset()
-            obs.append(o.copy())
-    _equal_records(ref, dict(obs=np.array(obs), reward=np.array(rew), done=np.array(done), counter=np.array(counter), ratio=np.array(ratio)))
+    got = _lockstep_record(orc, c, c.get("pseed", 8800), 4, c["steps"])
+    _equal_records({k: G["case_%s_%s" % (name, k)] for k in got}, got)
 
 
 @pytest.mark.parametrize("name", sorted(CONT_CASES))
 def test_continuous_cases_lockstep_with_reference(name):
-    import make_golden_cases as M
     from harness import cont_case_stream
     from pct_oracle import OracleContinuous
-    _, Cm = ref_shim.load_reference()
-    c = dict(CONT_CASES[name], steps=70)
-    ref = M.record_cont_case(Cm, c, 8801, 5)
+    c = dict(CONT_CASES[name], steps=CONT_CASE_STEPS)
     orc = OracleContinuous(c["setting"], container_size=c["container"], internal_node_holder=c["nb"], leaf_node_holder=c["nl"],
                            size_minimum=c["low"], stream=cont_case_stream(c, 8801, 5, c["steps"] + 64))
-    o = orc.reset()
-    obs, rew, done, counter, ratio = [o.copy()], [], [], [], []
-    for t in range(c["steps"]):
-        o, r, d, info = orc.step(ref["rows"][t])
-        obs.append(o.copy()); rew.append(r); done.append(d); counter.append(info["counter"]); ratio.append(info.get("ratio", -1.0))
-        if d:
-            o = orc.reset()
-            obs.append(o.copy())
-    _equal_records(ref, dict(obs=np.array(obs), reward=np.array(rew), done=np.array(done), counter=np.array(counter), ratio=np.array(ratio)))
+    got = _lockstep_record(orc, c, 8801, 5, c["steps"])
+    _equal_records({k: G["ccase_%s_%s" % (name, k)] for k in got}, got)
 
 
 def test_the_known_divergence_is_lapack_rounding_at_a_geometric_tie():
-    """The one disagreement a 130k-env-step fresh-seed soak found (scratch/soak_oracle_vs_reference.py; setting 1, seed 135409): a 4x2x1
-    item resting on three boxes whose common edge passes exactly under its centre of mass -> no direct edge -> np.linalg.lstsq (LAPACK
-    gelsd) splits the load.  The oracle's solver agrees with gelsd to 4e-16, but the next box's centre of mass then lies exactly ON the
-    border between two of ITS supports, and the strict `centre > area` tests (D:space.py:186-187) are decided by that last bit.
-    Demonstrated on the reference's own code: feed it the oracle solver's solution instead of LAPACK's and ITS verdict flips too.
-    (gelsd's last bits depend on the BLAS build, so this tie is not reproducible across machines even by the reference itself.)"""
+    """The one disagreement a 130k-env-step fresh-seed soak found (setting 1, seed 135409): a 4x2x1 item resting on three boxes whose
+    common edge passes exactly under its centre of mass -> no direct edge -> np.linalg.lstsq (LAPACK gelsd) splits the load.  The oracle's
+    solver agrees with gelsd to 4e-16, but the next box's centre of mass then lies exactly ON the border between two of ITS supports, and
+    the strict `centre > area` tests (D:space.py:186-187) are decided by that last bit.  Demonstrated on the reference's own code when the
+    record was made: fed the oracle solver's solution instead of LAPACK's, ITS verdict flips too.  (gelsd's last bits depend on the BLAS
+    build, so this tie is not reproducible across machines even by the reference itself.)"""
     from harness import case_stream
-    from pct_oracle import _dp, lib
-    D, _ = ref_shim.load_reference()
-    import pct_envs.PctDiscrete0.space as SP
-    c, seed, env_id = CASES["holders_s1"], 135409, 0
-    stream = case_stream(c, seed, env_id, 200)
-    ref = D.PackingDiscrete(setting=1, container_size=[10, 10, 10], item_set=c["items"], internal_node_holder=c["nb"], leaf_node_holder=c["nl"],
-                            shuffle=False, LNES="EMS")
-    ref.box_creator = ref_shim.make_stream_creator(D, [tuple(int(v) for v in r[:3]) for r in stream])
-    ref.test = True
-    orc = OracleDiscrete(1, internal_node_holder=c["nb"], leaf_node_holder=c["nl"], stream=stream)
-    o1, o2 = ref.reset(), orc.reset()
-    for t in range(47):
-        assert np.array_equal(o1, o2), t
-        _, row = policy_pick(o1, c["nb"], c["nl"], seed, env_id, t)
-        o1, _, d1, _ = ref.step(row)
-        o2, _, _, _ = orc.step(row)
-        if d1:
-            o1, o2 = ref.reset(), orc.reset()
-    lapack, L = np.linalg.lstsq, lib()
-    seen = []
-
-    def with_oracle_solver(A, b, rcond=None):
-        r = lapack(A, b, rcond=rcond)
-        x = np.zeros(A.shape[1])
-        L.pcto_lstsq(_dp(np.ascontiguousarray(A, dtype=float)), A.shape[0], A.shape[1], _dp(np.ascontiguousarray(np.array(b, dtype=float).reshape(-1))), _dp(x))
-        seen.append(np.abs(r[0].reshape(-1) - x).max())
-        return (x.reshape(-1, 1),) + tuple(r[1:])
-
-    args = ([4, 2, 1], (5, 0), False, ref.next_den, 1)
-    assert ref.space.drop_box_virtual(*args) is False  # LAPACK's last bits: infeasible
-    SP.np.linalg.lstsq = with_oracle_solver
-    try:
-        flipped = ref.space.drop_box_virtual(*args)
-    finally:
-        SP.np.linalg.lstsq = lapack
-    if not np.array_equal(o1, o2):  # on this machine's BLAS the tie falls the other way for the oracle: the documented divergence
-        assert flipped is True and len(seen) == 1 and 0 < seen[0] < 1e-15
+    c = CASES["holders_s1"]
+    orc = OracleDiscrete(1, internal_node_holder=c["nb"], leaf_node_holder=c["nl"], stream=case_stream(c, TIE_SEED, TIE_ENV, 200))
+    o = orc.reset()
+    for t in range(TIE_STEPS):
+        assert obs_digest(o) == G["tie_pre"][t], t
+        _, row = policy_pick(o, c["nb"], c["nl"], TIE_SEED, TIE_ENV, t)
+        o, _, d, _ = orc.step(row)
+        if d:
+            o = orc.reset()
+    assert not G["tie_with_lapack"][0]  # LAPACK's last bits: infeasible
+    if obs_digest(o) != G["tie_final"][0]:  # on this machine's BLAS the tie falls the other way for the oracle: the documented divergence
+        gap = G["tie_solver_gap"]
+        assert G["tie_with_oracle_solver"][0] and len(gap) == 1 and 0 < gap[0] < 1e-15

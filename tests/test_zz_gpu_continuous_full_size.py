@@ -2,8 +2,6 @@
 item generator) stepped with the synthetic policy — every one of the final float64 observations, the per-env episode counts and the
 reward sums must equal the threaded CPU oracle's (oracle/pct_oracle_batch_continuous.c).  Trajectories are chaotic, so equality of
 the final state certifies every intermediate step.  Settings 1 (stability) and 2 (six orientations).
-
-Green on a B200 (driver GPUTEST_r01 and round 2).
 """
 import numpy as np
 import pytest

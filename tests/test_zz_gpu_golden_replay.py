@@ -5,7 +5,7 @@ single-env facades (PackingDiscrete / PackingContinuous = a GPU batch of one, gy
 rows; every float64 observation — terminal ones and the ones after reset() included —, reward, done, counter and ratio
 must equal the record.
 
-Green on a B200 (driver GPUTEST_r01 and round 2).  No record is excluded.
+No record is excluded.
 """
 import glob
 import os

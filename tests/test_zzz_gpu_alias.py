@@ -2,7 +2,7 @@
 pct_apply_kernel<STAB, ALIAS = true> -> stability_check<true, GeomD, true>, the reference's Python-object semantics of the load entries,
 DESIGN.md section 3 (b)) against the oracle's alias mode — on the BASELINE-stream trajectories where the two semantics part
 (scratch/alias_rate.py) and on ordinary batches; the snapshot kernels must keep following the snapshot oracle on the same trajectories.
-Green on a B200 (driver GPUTEST_r01, round 2 call 1).  The routine's logic is also verified on its HOST build (tests/test_host_emul_stability.py).
+The routine's logic is also verified on its HOST build (tests/test_host_emul_stability.py).
 """
 import numpy as np
 import pytest

@@ -2,7 +2,7 @@
 csrc/pct_continuous.cu rest_height_pre) must be bit-identical to the default: same lock-step parity against the CPU oracle
 as tests/test_gpu_continuous_parity.py, and identical streams with the switch on and off.
 
-Green on a B200 (driver GPUTEST_r01; round 2: the pre-rounded loop is the default, +2 %).
+Round 2 made the pre-rounded loop the default.
 """
 import numpy as np
 import pytest

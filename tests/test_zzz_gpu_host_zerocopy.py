@@ -1,7 +1,7 @@
 """GPU: the zero-copy (default since round 2) observation delivery of pct_step_host (PCT_B200_HOST_ZEROCOPY=1: the kernels write the observation
 straight into the pinned host buffer) must return exactly what the staged path returns, and fall back to it for unpinned buffers.
 
-Green on a B200 (driver GPUTEST_r01; round 2: zero-copy is the default of pct_step_host, measured 5.2 -> 9.1 M env-steps/s with delta rows).
+Zero-copy is the default of pct_step_host.
 """
 import numpy as np
 import pytest

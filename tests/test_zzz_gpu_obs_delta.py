@@ -3,7 +3,7 @@ same observation buffer, only the rows that can differ from its contents are wri
 path writes — on the library-owned buffer, with alternating caller buffers (every switch falls back to a full write), inside a captured
 CUDA graph, and through the zero-copy host path.
 
-Green on a B200 (driver GPUTEST_r01; round 2: the delta rows are the default, this file also pins the full-rewrite mode).
+The delta rows are the default; this file also pins the full-rewrite mode.
 """
 import numpy as np
 import pytest
