@@ -62,7 +62,8 @@ enum pct_env_flags {
     PCT_FLAG_CAND_OVERFLOW = 8,     /* candidate set exceeded the fixed capacity                           */
     PCT_FLAG_EDGE_OVERFLOW = 16,    /* support-edge pool exceeded the fixed capacity                       */
     PCT_FLAG_SUPPORT_OVERFLOW = 32, /* more supports under one box than the stability routine handles      */
-    PCT_FLAG_SYNC_TIMEOUT = 64      /* internal: a kernel gave up waiting for the previous stage of this env */
+    PCT_FLAG_SYNC_TIMEOUT = 64,     /* internal: a kernel gave up waiting for the previous stage of this env */
+    PCT_FLAG_BAD_SNAPSHOT = 128     /* pct_restore was given a record of another configuration; the env was left as it was   */
 };
 
 /* Constructor arguments = the kwargs of PackingDiscrete / PackingContinuous.__init__
@@ -190,6 +191,36 @@ int pct_query_placement(pct_handle h, int32_t env, const int32_t dims[3], int32_
  * ONE env; synchronous.  rest_height is interSect2D's max_h (C:space.py:391). */
 int pct_query_placement_f64(pct_handle h, int32_t env, const double dims[3], double lx, double ly, double density,
                             int32_t *feasible, double *rest_height);
+
+/* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
+ * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
+ * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).
+ *
+ * A record holds exactly the state that carries over from one step to the next (what a step reads before it writes it: the placed
+ * boxes, EMS list, load edges and support polygons, the leaf rows of the last observation, the next item and its draw position, the
+ * episode counters and sticky flags, the alias-mode load objects and the LSAH footprint of pct_heuristic_actions*) and nothing
+ * transient.  It holds no pointers and no slot-dependent data, so it restores into any slot of any handle with the same
+ * configuration, on any device: moving or saving records is a plain byte copy.  Only the live parts of a record are written / read;
+ * the record size is fixed per domain so that records can be indexed.  A record starts with a 16-byte header: a layout version and
+ * a fingerprint of domain, setting, container, holder sizes, lnes and alias mode.
+ *
+ * Item source after a restore: the env keeps the record's draw position, but later items come from the slot it now occupies (its
+ * own counter-based key in PCT_ITEMS_RANDOM mode, its own stream row, with the trajectory length, in PCT_ITEMS_STREAM mode).  So
+ * children of one record restored into different slots sample different futures; a restore into the same slot, or into a slot
+ * with the same stream row and global env id, replays exactly the same future. */
+/* bytes of one record in a snapshot buffer of this handle (fixed per domain) */
+int64_t pct_snapshot_bytes(pct_handle h);
+/* gather: record i of d_buf (16-byte aligned, n x pct_snapshot_bytes) <- state of env d_env[i] (d_env NULL: envs 0..n-1).
+ * An index outside [0, n_envs) writes a header that no restore accepts. */
+int pct_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, void *stream);
+/* scatter: env d_env[i] <- record d_rec[i] of d_buf (d_env NULL: env i; d_rec NULL: record i; one record may feed many envs = fan-out).
+ *   Destinations within one call must be distinct (caller's contract).  Env indices outside [0, n_envs) and negative record indices
+ *   are skipped; record indices must address records inside d_buf.  A record whose header does not match this handle is not applied:
+ *   the env stays as it was and gets the sticky PCT_FLAG_BAD_SNAPSHOT, which its next step reports.
+ *   d_obs non-NULL: writes the COMPLETE observation rows of every restored env into d_obs (row layout of pct_step, row = env index).
+ *   Delta rows: a restored env's next pct_step rewrites all of its rows in whatever buffer it receives, so restoring with d_obs NULL
+ *   keeps the observation-buffer contract of pct_step. */
+int pct_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_t n, const void *d_buf, void *d_obs, void *stream);
 
 /* introspection */
 int pct_get_state(pct_handle h, int32_t env, pct_state_dump *out);

@@ -62,6 +62,7 @@ class PctBatch(object):
         cfg.lnes = _lib.LNES_CODES[LNES]
         cfg.shuffle = int(bool(shuffle))
         self.cfg = cfg
+        self.did_reset = False
         h = C.c_void_p()
         rc = self.L.pct_create(C.byref(cfg), self.n_envs, int(device), C.byref(h))
         if rc != 0:
@@ -111,6 +112,7 @@ class PctBatch(object):
     def reset(self, out=None):
         obs = self._obs if out is None else out
         self._check(self.L.pct_reset(self.h, C.c_void_p(obs.data_ptr()), self._stream()), "pct_reset")
+        self.did_reset = True
         return obs
 
     def step(self, actions=None, leaf_idx=None, out=None):
@@ -147,6 +149,64 @@ class PctBatch(object):
         self._check(self.L.pct_policy_random_dev(self.h, C.c_void_p(idx.data_ptr()), int(seed) & ((1 << 64) - 1), C.c_void_p(t_dev.data_ptr()),
                                                  self._stream()), "pct_policy_random_dev")
         return idx
+
+    # -- snapshot / restore (include/pct_b200.h) --------------------------------------------------------------
+    @property
+    def snapshot_bytes(self):
+        """bytes of one env record (fixed per domain)"""
+        return int(self.L.pct_snapshot_bytes(self.h))
+
+    def _index(self, idx, what):
+        if idx is None:
+            return None
+        if not torch.is_tensor(idx):
+            idx = torch.as_tensor(np.asarray(idx, dtype=np.int32))
+        if idx.dim() != 1:
+            raise PctError("%s must be one-dimensional" % what)
+        return idx.to(device=self.device, dtype=torch.int32).contiguous()
+
+    def snapshot(self, env_idx=None, out=None):
+        """State records of envs `env_idx` (default: every env) -> (n, snapshot_bytes) uint8 CUDA tensor, filled on the current stream.
+        The records hold no pointers: they can be moved to another GPU, saved and restored into any slot of a batch with the same
+        configuration (restore)."""
+        idx = self._index(env_idx, "env_idx")
+        n = self.n_envs if idx is None else int(idx.numel())
+        B = self.snapshot_bytes
+        if out is None:
+            out = torch.empty((n, B), dtype=torch.uint8, device=self.device)
+        elif out.dtype != torch.uint8 or out.device != self.device or not out.is_contiguous() or tuple(out.shape) != (n, B):
+            raise PctError("snapshot out must be a contiguous (%d, %d) uint8 tensor on %s" % (n, B, self.device))
+        self._check(self.L.pct_snapshot(self.h, C.c_void_p(idx.data_ptr()) if idx is not None else None, n, C.c_void_p(out.data_ptr()),
+                                        self._stream()), "pct_snapshot")
+        return out
+
+    def restore(self, snap, env_idx=None, rec_idx=None, out=None, write_obs=True):
+        """Env env_idx[i] <- record rec_idx[i] of `snap` (defaults: env i, record i; one record may feed many envs).  Destinations must be
+        distinct.  Record indices outside `snap` are skipped (on the device, without a synchronisation).  Writes the complete observation
+        rows of the restored envs into `out` (default: the batch's own observation buffer) and returns it; write_obs=False writes no rows
+        (the next step then rewrites every row of the restored envs) and returns None.  A record of another configuration leaves its env
+        unchanged and flags it (bad_snapshot, reported by the next step)."""
+        if snap.dtype != torch.uint8 or snap.dim() != 2 or snap.shape[1] != self.snapshot_bytes:
+            raise PctError("snapshot must be an (n, %d) uint8 tensor" % self.snapshot_bytes)
+        snap = snap.to(self.device).contiguous()
+        env = self._index(env_idx, "env_idx")
+        rec = self._index(rec_idx, "rec_idx")
+        n = int(env.numel()) if env is not None else (int(rec.numel()) if rec is not None else int(snap.shape[0]))
+        if rec is not None:
+            if int(rec.numel()) != n:
+                raise PctError("env_idx and rec_idx must have the same length")
+            rec = torch.where((rec >= 0) & (rec < snap.shape[0]), rec, torch.full_like(rec, -1))
+        elif n > snap.shape[0]:
+            raise PctError("restore of %d envs from %d records without rec_idx" % (n, snap.shape[0]))
+        obs = None
+        if write_obs:
+            obs = self._obs if out is None else out
+            if obs.dtype != self.obs_dtype or not obs.is_contiguous() or tuple(obs.shape) != (self.n_envs, self.obs_len):
+                raise PctError("restore out must be a contiguous (n_envs, obs_len) tensor of the batch's observation dtype")
+        self._check(self.L.pct_restore(self.h, C.c_void_p(env.data_ptr()) if env is not None else None,
+                                       C.c_void_p(rec.data_ptr()) if rec is not None else None, n, C.c_void_p(snap.data_ptr()),
+                                       C.c_void_p(obs.data_ptr()) if obs is not None else None, self._stream()), "pct_restore")
+        return obs
 
     # -- heuristic baselines (heuristic.py) ------------------------------------------------------------------
     def heuristic_actions(self, name, seed=0, t=0, out=None):
@@ -191,6 +251,7 @@ class PctBatch(object):
     # -- host-buffer API (what the reference's VecEnv exchanges over its pipes) --------------------------------
     def reset_host(self, obs_out):
         self._check(self.L.pct_reset_host(self.h, C.c_void_p(obs_out.ctypes.data)), "pct_reset_host")
+        self.did_reset = True
         return obs_out
 
     def step_host(self, obs_out, rew_out, done_out, info_out=None, actions=None, leaf_idx=None):

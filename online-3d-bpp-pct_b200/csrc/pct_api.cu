@@ -34,6 +34,11 @@ int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out);
 int64_t continuous_state_bytes();
 int continuous_heuristic(pct_env_batch *h, int code, double *rows, double *hstate, cudaStream_t st);
 int continuous_query(pct_env_batch *h, int env, const double q[5], double density, double *d_out, cudaStream_t st);
+// snapshot / restore (pct_snapshot.cu)
+int64_t snapshot_record_bytes(const pct_env_batch *h);
+uint64_t snapshot_fingerprint(const pct_env_batch *h);
+cudaError_t launch_snapshot(pct_env_batch *h, const int32_t *env, int n, void *buf, cudaStream_t st);
+cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, void *obs, cudaStream_t st);
 }  // namespace pct
 
 extern "C" {
@@ -121,6 +126,15 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
         e = cudaStreamCreateWithPriority(&h->sub[gi], cudaStreamNonBlocking, prio_of(gi));
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->ev_join[gi], cudaEventDisableTiming);
     }
+    // LSAH footprint rows (pct_heuristic_actions*): allocated here so that pct_snapshot / pct_restore, which move them, never allocate
+    if (e == cudaSuccess && cfg->domain == PCT_DISCRETE) {
+        e = cudaMalloc(&h->d_hstate, sizeof(int32_t) * 4 * (size_t)n_envs);
+        if (e == cudaSuccess) e = cudaMemset(h->d_hstate, 0, sizeof(int32_t) * 4 * (size_t)n_envs);
+    } else if (e == cudaSuccess) {
+        e = cudaMalloc(&h->d_hstate_c, sizeof(double) * 4 * (size_t)n_envs);
+        if (e == cudaSuccess) e = cudaMemset(h->d_hstate_c, 0, sizeof(double) * 4 * (size_t)n_envs);
+    }
+    h->snap_fp = snapshot_fingerprint(h);
     if (e == cudaSuccess) {
         if (cfg->domain == PCT_DISCRETE) {
             e = cudaMalloc(&h->d_hot, sizeof(DEnvHot) * (size_t)n_envs);
@@ -486,10 +500,6 @@ int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64
         h->err = "PCT_H_HM / PCT_H_MACS / PCT_H_RANDOM need container sides <= 32";
         return PCT_ERR_INVALID;
     }
-    if (!h->d_hstate) {
-        CK(h, cudaMalloc(&h->d_hstate, sizeof(int32_t) * 4 * (size_t)h->n_envs));
-        CK(h, cudaMemset(h->d_hstate, 0, sizeof(int32_t) * 4 * (size_t)h->n_envs));
-    }
     HParams hp{};
     hp.code = heuristic; hp.rows = d_rows; hp.hstate = h->d_hstate; hp.seed = seed; hp.t = t;
     CK(h, launch_heuristic_discrete(p, hp, (cudaStream_t)stream));
@@ -507,10 +517,6 @@ int pct_heuristic_actions_f64(pct_handle h, int32_t heuristic, double *d_rows, v
     if (!h->did_reset) { h->err = "pct_heuristic_actions_f64 before pct_reset"; return PCT_ERR_STATE; }
     if (heuristic == PCT_H_BR && !h->d_item_set) { h->err = "PCT_H_BR scores an EMS by the item types that fit: call pct_set_item_set"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
-    if (!h->d_hstate_c) {
-        CK(h, cudaMalloc(&h->d_hstate_c, sizeof(double) * 4 * (size_t)h->n_envs));
-        CK(h, cudaMemset(h->d_hstate_c, 0, sizeof(double) * 4 * (size_t)h->n_envs));
-    }
     int rc = continuous_heuristic(h, heuristic, d_rows, h->d_hstate_c, (cudaStream_t)stream);
     if (rc != PCT_OK) return rc;
     h->launches++;
@@ -582,6 +588,30 @@ int pct_get_state(pct_handle h, int32_t env, pct_state_dump *out) {
     }
     for (int i = 0; i < hot.h.n_ems && i < 256 && i < E_MAX; i++)
         for (int t = 0; t < 6; t++) out->ems[i][t] = hot.ems[i][t];
+    return PCT_OK;
+}
+
+int64_t pct_snapshot_bytes(pct_handle h) { return h ? snapshot_record_bytes(h) : 0; }
+
+int pct_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    if (!d_buf || n < 0 || ((uintptr_t)d_buf & 15)) { h->err = "pct_snapshot: d_buf must be a 16-byte aligned device buffer and n >= 0"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_snapshot before pct_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    CK(h, cudaSetDevice(h->device));
+    CK(h, launch_snapshot(h, d_env, n, d_buf, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
+int pct_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_t n, const void *d_buf, void *d_obs, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    if (!d_buf || n < 0 || ((uintptr_t)d_buf & 15)) { h->err = "pct_restore: d_buf must be a 16-byte aligned device buffer and n >= 0"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_restore before pct_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    CK(h, cudaSetDevice(h->device));
+    CK(h, launch_restore(h, d_env, d_rec, n, d_buf, d_obs, (cudaStream_t)stream));
+    h->launches++;
     return PCT_OK;
 }
 

@@ -41,8 +41,9 @@ struct pct_env_batch {
     bool fill_pending = false;
     bool host_zero_copy = true;   // pct_step_host: kernels write the observation straight into the pinned (mapped) host buffer; PCT_B200_HOST_ZEROCOPY=0: staged copies
     bool cont_pre = true;         // continuous feas_emit: resting heights from pre-rounded rectangles (exact; PCT_B200_CONT_PRE=0 disables)
-    int32_t *d_hstate = nullptr;  // (n_envs, 4) LSAH footprint state (pct_heuristic_actions)
+    int32_t *d_hstate = nullptr;  // (n_envs, 4) LSAH footprint state (pct_heuristic_actions; discrete handles)
     double *d_hstate_c = nullptr; // same for the continuous domain (pct_heuristic_actions_f64)
+    uint64_t snap_fp = 0;         // fingerprint written into / required of snapshot records (pct_snapshot.cu)
     double *d_query_c = nullptr;  // 2 doubles: result of pct_query_placement_f64
     int32_t *d_query = nullptr;   // 2 + W*L ints: result of pct_query_placement
     int item_mode = 0;

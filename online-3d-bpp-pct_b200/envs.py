@@ -9,6 +9,8 @@ observations as the reference returns them), so `evaluation_tools.evaluate` (eva
 heuristics' read-only attribute accesses work unchanged.  They exist for drop-in compatibility; throughput comes
 from PctVecEnv / PctBatch.
 """
+import copy
+
 import numpy as np
 import torch
 
@@ -93,17 +95,40 @@ class _PackingBase(object):
             for i, t in enumerate(trajs):
                 seq[i, :len(t), :t.shape[1]] = t
             stream = seq.reshape(1, -1, 4)
-        self._batch = PctBatch(1, setting, container_size=container_size, item_set=item_set, internal_node_holder=internal_node_holder,
-                               leaf_node_holder=leaf_node_holder, continuous=self._continuous, obs_dtype=torch.float64, seed=seed,
-                               device=device, sample_from_distribution=sample_from_distribution and self._continuous,
-                               sample_left_bound=sample_left_bound, sample_right_bound=sample_right_bound, item_stream=stream,
-                               size_minimum=size_minimum, auto_reset=False, LNES=LNES, shuffle=shuffle)
-        if traj_len:
-            self._batch.set_trajectory_length(traj_len)
+        # kept for __deepcopy__, which builds a second batch of one from the same arguments
+        self._batch_args = dict(container_size=container_size, item_set=item_set, internal_node_holder=internal_node_holder,
+                                leaf_node_holder=leaf_node_holder, continuous=self._continuous, obs_dtype=torch.float64, seed=seed,
+                                device=device, sample_from_distribution=sample_from_distribution and self._continuous,
+                                sample_left_bound=sample_left_bound, sample_right_bound=sample_right_bound, item_stream=stream,
+                                size_minimum=size_minimum, auto_reset=False, LNES=LNES, shuffle=shuffle)
+        self._traj_len = traj_len
+        self._batch = self._new_batch()
         self.observation_space = _make_box(0.0, float(container_size[2]), (self._batch.obs_len,))
         self.space = _SpaceView(self)
         self.SEED = seed
         self._next_box_override = None
+
+    def _new_batch(self):
+        b = PctBatch(1, self.setting, **self._batch_args)
+        if self._traj_len:
+            b.set_trajectory_length(self._traj_len)
+        return b
+
+    def __deepcopy__(self, memo):
+        """copy.deepcopy(env), as on the reference's plain-Python env: an independent env in the same state.  The copy is env 0 of its own
+        batch with the same arguments, so it continues with exactly the items the original would draw."""
+        new = type(self).__new__(type(self))
+        memo[id(self)] = new
+        for k, v in self.__dict__.items():
+            if k not in ("_batch", "_batch_args", "space"):
+                setattr(new, k, copy.deepcopy(v, memo))
+        new._batch_args = self._batch_args  # read-only after construction
+        new._batch = new._new_batch()
+        new.space = _SpaceView(new)
+        if self._batch.did_reset:
+            new._batch.reset()
+            new._batch.restore(self._batch.snapshot())
+        return new
 
     # ---- gym.Env API ----
     def seed(self, seed=None):  # D:bin3D.py:47-54 (the item generator is counter-based: the seed is fixed at construction)
