@@ -192,6 +192,30 @@ int pct_query_placement(pct_handle h, int32_t env, const int32_t dims[3], int32_
 int pct_query_placement_f64(pct_handle h, int32_t env, const double dims[3], double lx, double ly, double density,
                             int32_t *feasible, double *rest_height);
 
+/* Batched placement queries: Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) (D:space.py:393-433,
+ * C:space.py:380-425) for many placements of many envs — the primitive for placement rules of one's own (a heuristic, a learned critic
+ * over candidate placements, a search on branched envs).  Row r asks k placements of env d_env[r] (d_env NULL: env r).
+ *   d_q        : n x k x 5 placements [x, y, z, lx, ly]; x, y, z are the oriented sizes (int32 discrete / float64 continuous)
+ *   d_density  : n x k densities, or NULL = each env's current item density (what the facades' drop_box_virtual passes)
+ *   d_feasible : n x k uint8;  d_rest_height: n x k int32 / float64 (either output may be NULL)
+ * Every answer equals what pct_query_placement(_f64) returns for the same env and inputs, bit for bit, degenerate inputs included: a
+ * discrete position outside [0, W) x [0, L) or a zero x / y is infeasible with rest height 0; a footprint that sticks out of the
+ * container is infeasible with its rest height still reported; the continuous bounds carry the reference's 1e-6 tolerances.
+ * Read-only: env state, sticky flags, the delta-row bookkeeping and the LSAH footprint are untouched (capacity flags of the stability
+ * test are not reported), so a step after a query behaves exactly as without it.  Enqueue only: no host synchronisation, no
+ * allocation (CUDA-graph capturable).  The env indices of one call must be distinct (caller's contract, as for pct_restore: the
+ * stability test of an env uses that env's scratch); a row whose index is outside [0, n_envs) gets feasible 0 and rest height 0.
+ * k has no cap, and no container limit applies beyond pct_create's.  n == 0 or k == 0: no-op.  Errors: PCT_ERR_STATE before
+ * pct_reset; PCT_ERR_INVALID for the other domain, n < 0, k < 0 or n * k > INT32_MAX. */
+int pct_query_placements(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, const int32_t *d_q, const double *d_density,
+                         uint8_t *d_feasible, int32_t *d_rest_height, void *stream);   /* discrete   */
+int pct_query_placements_f64(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, const double *d_q, const double *d_density,
+                             uint8_t *d_feasible, double *d_rest_height, void *stream); /* continuous */
+/* Space.plain[:W, :L] (D:space.py:278, 317-326), the height map, of envs d_env[0..n) (d_env NULL: 0..n-1) -> d_out, n x W x L int32
+ * (row-major).  Discrete only: the continuous Space has no height map.  An index outside [0, n_envs) gives a zero map.  Same
+ * enqueue-only, read-only and error contract as pct_query_placements; no container side limit. */
+int pct_height_maps(pct_handle h, const int32_t *d_env, int32_t n, int32_t *d_out, void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

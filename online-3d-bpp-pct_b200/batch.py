@@ -248,6 +248,64 @@ class PctBatch(object):
                                                hm.ctypes.data_as(C.POINTER(C.c_int32)) if want_map else None), "pct_query_placement")
         return (bool(feas.value), mh.value, hm) if want_map else (bool(feas.value), mh.value)
 
+    # -- batched placement queries and height maps (include/pct_b200.h) --------------------------------------------
+    def _out(self, t, shape, dtype, what):
+        if not torch.is_tensor(t) or t.dtype != dtype or t.device != self.device or not t.is_contiguous() or tuple(t.shape) != shape:
+            raise PctError("%s must be a contiguous %s %s tensor on %s" % (what, shape, dtype, self.device))
+        return t
+
+    def query_placements(self, queries, env_idx=None, density=None, out=None):
+        """Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) (D:space.py:393-433, C:space.py:380-425) for k
+        placements of each of n envs, enqueued on the current stream (graph-capturable, read-only: a step after a query behaves as without it).
+        queries: (n, k, 5) tensor of [x, y, z, lx, ly] (oriented sizes, then the position), converted to int32 (discrete) / float64
+        (continuous) on the batch's device.  Row r asks env env_idx[r] (default: env r); the envs of one call must be distinct, and rows of
+        an index outside [0, n_envs) answer infeasible / 0.  density: (n, k) densities (default: each env's current item density).
+        out: optional preallocated (feasible, rest_height) pair.  -> (feasible (n, k) bool, rest_height (n, k) int32 | float64)."""
+        qd = torch.float64 if self.continuous else torch.int32
+        if not torch.is_tensor(queries):
+            queries = torch.as_tensor(np.asarray(queries))
+        if queries.dim() != 3 or queries.shape[2] != 5:
+            raise PctError("queries must have shape (n, k, 5): [x, y, z, lx, ly] per placement")
+        n, k = int(queries.shape[0]), int(queries.shape[1])
+        q = queries.to(device=self.device, dtype=qd).contiguous()
+        idx = self._index(env_idx, "env_idx")
+        if idx is not None and int(idx.numel()) != n:
+            raise PctError("env_idx must have one entry per query row (%d)" % n)
+        if idx is None and n > self.n_envs:
+            raise PctError("%d query rows without env_idx for %d envs" % (n, self.n_envs))
+        den = None
+        if density is not None:
+            if not torch.is_tensor(density):
+                density = torch.as_tensor(np.asarray(density, dtype=np.float64))
+            if tuple(density.shape) != (n, k):
+                raise PctError("density must have shape (n, k) = (%d, %d)" % (n, k))
+            den = density.to(device=self.device, dtype=torch.float64).contiguous()
+        if out is None:
+            feas = torch.empty((n, k), dtype=torch.bool, device=self.device)
+            rest = torch.empty((n, k), dtype=qd, device=self.device)
+        else:
+            if len(out) != 2:
+                raise PctError("out must be a (feasible, rest_height) pair")
+            feas = self._out(out[0], (n, k), torch.bool, "out[0] (feasible)")
+            rest = self._out(out[1], (n, k), qd, "out[1] (rest_height)")
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
+        fn, what = (self.L.pct_query_placements_f64, "pct_query_placements_f64") if self.continuous else (self.L.pct_query_placements, "pct_query_placements")
+        self._check(fn(self.h, ptr(idx), n, k, ptr(q), ptr(den), ptr(feas), ptr(rest), self._stream()), what)
+        return feas, rest
+
+    def height_maps(self, env_idx=None, out=None):
+        """Space.plain[:W, :L] (D:space.py:278, 317-326), the height map, of envs env_idx (default: every env) -> (n, W, L) int32 CUDA
+        tensor, filled on the current stream (graph-capturable, read-only).  Indices outside [0, n_envs) give a zero map.  Discrete only."""
+        if self.continuous:
+            raise PctError("height_maps: the continuous Space has no height map (discrete domain only)")
+        idx = self._index(env_idx, "env_idx")
+        n = self.n_envs if idx is None else int(idx.numel())
+        shape = (n, int(self.container_size[0]), int(self.container_size[1]))
+        out = torch.empty(shape, dtype=torch.int32, device=self.device) if out is None else self._out(out, shape, torch.int32, "height_maps out")
+        self._check(self.L.pct_height_maps(self.h, C.c_void_p(idx.data_ptr()) if idx is not None and n else None, n,
+                                           C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_height_maps")
+        return out
+
     # -- host-buffer API (what the reference's VecEnv exchanges over its pipes) --------------------------------
     def reset_host(self, obs_out):
         self._check(self.L.pct_reset_host(self.h, C.c_void_p(obs_out.ctypes.data)), "pct_reset_host")

@@ -34,6 +34,7 @@ int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out);
 int64_t continuous_state_bytes();
 int continuous_heuristic(pct_env_batch *h, int code, double *rows, double *hstate, cudaStream_t st);
 int continuous_query(pct_env_batch *h, int env, const double q[5], double density, double *d_out, cudaStream_t st);
+int continuous_queries(pct_env_batch *h, const QParams &q, cudaStream_t st);
 // snapshot / restore (pct_snapshot.cu)
 int64_t snapshot_record_bytes(const pct_env_batch *h);
 uint64_t snapshot_fingerprint(const pct_env_batch *h);
@@ -565,6 +566,58 @@ int pct_query_placement(pct_handle h, int32_t env, const int32_t dims[3], int32_
     *feasible = out[0];
     *rest_height = out[1];
     if (height_map) memcpy(height_map, out.data() + 2, sizeof(int32_t) * cells);
+    return PCT_OK;
+}
+
+// argument checks shared by the two batched query calls; PCT_OK with n == 0 or k == 0 means "nothing to do" to the caller
+static int check_queries(pct_handle h, const char *what, int domain, int32_t n, int32_t k, const void *d_q) {
+    if (h->cfg.domain != domain) {
+        h->err = std::string(what) + (domain == PCT_DISCRETE ? ": discrete domain only (continuous: pct_query_placements_f64)"
+                                                             : ": continuous domain only (discrete: pct_query_placements)");
+        return PCT_ERR_INVALID;
+    }
+    if (n < 0 || k < 0) { h->err = std::string(what) + ": n and k must be >= 0"; return PCT_ERR_INVALID; }
+    if ((int64_t)n * k > INT32_MAX) { h->err = std::string(what) + ": n * k overflows int32"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = std::string(what) + " before pct_reset"; return PCT_ERR_STATE; }
+    if (n > 0 && k > 0 && !d_q) { h->err = std::string(what) + ": d_q is NULL"; return PCT_ERR_INVALID; }
+    return PCT_OK;
+}
+
+int pct_query_placements(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, const int32_t *d_q, const double *d_density,
+                         uint8_t *d_feasible, int32_t *d_rest_height, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    const int rc = check_queries(h, "pct_query_placements", PCT_DISCRETE, n, k, d_q);
+    if (rc != PCT_OK || n == 0 || k == 0) return rc;
+    CK(h, cudaSetDevice(h->device));
+    const QParams q{d_env, n, k, d_q, d_density, d_feasible, d_rest_height};
+    CK(h, launch_queries_discrete(state_params(h), q, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
+int pct_query_placements_f64(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, const double *d_q, const double *d_density,
+                             uint8_t *d_feasible, double *d_rest_height, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_queries(h, "pct_query_placements_f64", PCT_CONTINUOUS, n, k, d_q);
+    if (rc != PCT_OK || n == 0 || k == 0) return rc;
+    CK(h, cudaSetDevice(h->device));
+    const QParams q{d_env, n, k, d_q, d_density, d_feasible, d_rest_height};
+    rc = continuous_queries(h, q, (cudaStream_t)stream);
+    if (rc != PCT_OK) return rc;
+    h->launches++;
+    return PCT_OK;
+}
+
+int pct_height_maps(pct_handle h, const int32_t *d_env, int32_t n, int32_t *d_out, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    if (h->cfg.domain != PCT_DISCRETE) { h->err = "pct_height_maps: discrete domain only (the continuous Space has no height map)"; return PCT_ERR_INVALID; }
+    if (n < 0) { h->err = "pct_height_maps: n must be >= 0"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_height_maps before pct_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    if (!d_out) { h->err = "pct_height_maps: d_out is NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    CK(h, launch_height_maps(state_params(h), d_env, n, d_out, (cudaStream_t)stream));
+    h->launches++;
     return PCT_OK;
 }
 

@@ -1611,3 +1611,4 @@ cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_
 }  // namespace pct
 
 #include "pct_heuristics.cuh"
+#include "pct_query.cuh"

@@ -33,6 +33,30 @@ __device__ __forceinline__ void heur_rot(const int nb[3], int rot, int &x, int &
 
 struct HCand { int sx, sy, sz, lx, ly, ex, ey, ez; bool valid; };
 
+// Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) + check_box (D:space.py:393-454) of ONE placement
+// of a staged env, for the batched queries (pct_query.cuh).  It is the PCT_H_QUERY_ branch below, expression for expression (same
+// rest_height, same stability_check instantiation).  That branch keeps its own inline copy because routing it through this function
+// changes the register allocation of pct_heuristic_kernel; tests/test_gpu_queries.py pins the two paths to each other.  A position
+// outside [0, W) x [0, L) or a zero footprint is infeasible with rest height 0; a footprint that sticks out of the container is
+// infeasible with its rest height reported.  Raised capacity flags go to `fl` (the callers do not OR them into the env).
+template <bool STAB>
+__device__ __forceinline__ int query_placement_d(const DEnvHot *hot, int n_box, const GeomD &g, EdgePool &pool, BigScratch *big, int *lock,
+                                                 int W, int L, int H, int sx, int sy, int sz, int lx, int ly, double den, int &mh, int &fl) {
+    int feas = 0;
+    mh = 0;
+    if (lx >= 0 && ly >= 0 && lx < W && ly < L && sx > 0 && sy > 0) {
+        mh = rest_height(hot->box, 0, n_box, 1, lx, ly, lx + sx, ly + sy);
+        if (lx + sx > W || ly + sy > L) feas = 0;
+        else if (mh + sz > H) feas = 0;
+        else if (!STAB || mh == 0) feas = 1;
+        else {
+            NodeD root{lx, ly, mh, sx, sy, sz, (double)(sx * sy * sz) * den};
+            feas = stability_check<false, GeomD>(g, root, pool, big, lock, 0, fl) != 0;
+        }
+    }
+    return feas;
+}
+
 // enumeration index -> placement.  EMS family: ems (list order; OnlineBPH: deep-bottom-left order) x rot [x corner];
 // grid family: lx x ly x rot with the loop bounds of the UNROTATED item (heuristic.py:253-254).
 __device__ __forceinline__ HCand heur_decode(int code, int c, const int16_t (*ems)[6], const uint8_t *ord, const int nb[3], int R, int ny) {

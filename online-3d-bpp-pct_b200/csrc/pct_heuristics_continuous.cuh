@@ -31,6 +31,28 @@ __device__ __forceinline__ void heur_rot_c(const double nb[3], int rot, double &
 
 struct HCandC { double sx, sy, sz, lx, ly, ex, ey, ez; bool valid; };
 
+// Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) + check_box (C:space.py:380-439) of ONE placement:
+// for the batched queries (pctc_query_kernel).  It is the PCT_H_QUERY_ branch below, expression for expression; that branch keeps
+// its own inline copy because routing it through this function changes the register allocation of pctc_heuristic_kernel, and
+// tests/test_gpu_queries.py pins the two paths to each other.  mh is interSect2D's max_h (C:space.py:391), reported whatever the
+// verdict.  Raised capacity flags go to `fl` (the callers do not OR them into the env).
+template <bool STAB>
+__device__ __forceinline__ int query_placement_c(const CParams &p, const double (*box)[6], int n_box, const GeomC &g, EdgePool &pool, BigScratch *big,
+                                                 int *lock, double sx, double sy, double sz, double lx, double ly, double den, double &mh, int &fl) {
+    bool chk = !(lx + sx - 1e-6 > p.W || ly + sy - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
+    mh = rest_height_c(box, 0, n_box, 1, lx, ly, lx + sx, ly + sy);
+    if (mh < 0) mh = 0.0;
+    if (mh + sz - 1e-6 > p.H) chk = false;
+    int feas;
+    if (!chk) feas = 0;
+    else if (!STAB || fabs(mh) < 1e-6) feas = 1;
+    else {
+        NodeC root{lx, ly, mh, sx, sy, sz, sx * sy * sz * den};
+        feas = stability_check<false, GeomC>(g, root, pool, big, lock, 0, fl) != 0;
+    }
+    return feas;
+}
+
 // enumeration index -> placement: EMS (list order; OnlineBPH: deep-bottom-left order) x orientation, at the EMS origin
 __device__ __forceinline__ HCandC heur_decode_c(int code, int c, const double (*ems)[6], const uint16_t *ord, const double nb[3], int R) {
     HCandC k;
@@ -183,6 +205,47 @@ __global__ void __launch_bounds__(64) pctc_heuristic_kernel(const CParams p, con
     }
 }
 
+// Batched placement queries (pct_query_placements_f64): a block of 64 threads owns one row (k placements of one env, read in
+// place like pctc_heuristic_kernel does), one thread per placement of the current 64-chunk, answered by query_placement_c.  Nothing
+// is written back to the env.  Envs within one launch are distinct (caller's contract): stability_check uses the env's `big`
+// scratch under the block's lock.
+template <bool STAB>
+__global__ void __launch_bounds__(64) pctc_query_kernel(const CParams p, const QParams q) {
+    __shared__ int lock;
+    const int tid = threadIdx.x, r = blockIdx.x, K = q.k;
+    const int e = q.env ? q.env[r] : r;
+    const size_t row = (size_t)r * K;
+    double *rest = (double *)q.rest;
+    if (e < 0 || e >= p.n_envs) {  // not an env of this handle: infeasible, rest height 0
+        for (int j = tid; j < K; j += 64) {
+            if (q.feasible) q.feasible[row + j] = 0;
+            if (rest) rest[row + j] = 0.0;
+        }
+        return;
+    }
+    CEnv *ev = p.env + e;
+    const CHdr &h = ev->h;
+    if (tid == 0) lock = 0;
+    __syncthreads();
+    const int n_box = h.n_box;
+    GeomC g{ev->box, ev->den, n_box};
+    EdgePool pool{ev->e_lower, ev->e_next, ev->e_off, ev->first_in, ev->last_in, ev->e_st, ev->e_st, h.n_edge,
+                  ev->poly_off, &ev->poly[0][0], &ev->poly[0][0], h.n_poly};
+    int fl = 0;  // not ORed into the env: a query leaves the env as it was
+    const double *qv = (const double *)q.q;
+#pragma unroll 1
+    for (int base = 0; base < K; base += 64) {
+        const int j = base + tid;
+        if (j >= K) break;
+        const double *x = qv + (row + j) * 5;
+        const double den = q.density ? q.density[row + j] : h.next_den;
+        double mh;
+        const int feas = query_placement_c<STAB>(p, ev->box, n_box, g, pool, &ev->big, &lock, x[0], x[1], x[2], x[3], x[4], den, mh, fl);
+        if (q.feasible) q.feasible[row + j] = (uint8_t)feas;
+        if (rest) rest[row + j] = mh;
+    }
+}
+
 static CParams state_params_c(pct_env_batch *h) {
     CParams p{};
     p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs;
@@ -202,6 +265,15 @@ int continuous_query(pct_env_batch *h, int env, const double q[5], double densit
     else pctc_heuristic_kernel<true><<<1, 64, 0, st>>>(p, hp);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { h->err = std::string("continuous query launch: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
+    return PCT_OK;
+}
+
+int continuous_queries(pct_env_batch *h, const QParams &q, cudaStream_t st) {
+    const CParams p = state_params_c(h);
+    if (p.setting == 2) pctc_query_kernel<false><<<q.n, 64, 0, st>>>(p, q);
+    else pctc_query_kernel<true><<<q.n, 64, 0, st>>>(p, q);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { h->err = std::string("continuous queries launch: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
     return PCT_OK;
 }
 

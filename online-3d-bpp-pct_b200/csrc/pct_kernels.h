@@ -252,8 +252,21 @@ struct HParamsC {
     double *q_out;
 };
 constexpr int PCT_H_QUERY_ = 7;
-constexpr int HEUR_SIDE_MAX = 32;  // height-map based codes (HM, MACS, RANDOM's bitmap, queries): W, L <= 32
+constexpr int HEUR_SIDE_MAX = 32;  // height-map based codes (HM, MACS, RANDOM's bitmap, single discrete query): W, L <= 32
 cudaError_t launch_heuristic_discrete(const DParams &p, const HParams &hp, cudaStream_t st);
+
+// batched placement queries (pct_query.cuh; continuous: pct_heuristics_continuous.cuh): row r asks k placements of env env[r]
+struct QParams {
+    const int32_t *env;      // [n] env of row r, nullptr: env r
+    int n, k;
+    const void *q;           // n x k x 5 [x, y, z, lx, ly]: int32 (discrete) / float64 (continuous)
+    const double *density;   // n x k, nullptr: the env's current item density
+    uint8_t *feasible;       // n x k, or nullptr
+    void *rest;              // n x k rest heights, int32 (discrete) / float64 (continuous), or nullptr
+};
+cudaError_t launch_queries_discrete(const DParams &p, const QParams &q, cudaStream_t st);
+// Space.plain[:W, :L] of envs env[0..n) (nullptr: 0..n-1) -> out, n x W x L int32
+cudaError_t launch_height_maps(const DParams &p, const int32_t *env, int n, int32_t *out, cudaStream_t st);
 
 // delta observation writes: aux[i].obs_prev = {nb, nl} for n envs ("every row of the buffer may be non-zero")
 void launch_fill_prev(DEnvAux *aux, int n_envs, int nb, int nl, cudaStream_t st);
