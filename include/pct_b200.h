@@ -216,6 +216,40 @@ int pct_query_placements_f64(pct_handle h, const int32_t *d_env, int32_t n, int3
  * enqueue-only, read-only and error contract as pct_query_placements; no container side limit. */
 int pct_height_maps(pct_handle h, const int32_t *d_env, int32_t n, int32_t *d_out, void *stream);
 
+/* Item preview and item override: control over WHICH item an env packs, for lookahead ("online packing with lookahead": the agent
+ * knows the next k items) and buffer packing (the agent picks one of B buffered items, then places it).  Both calls only enqueue
+ * kernels on `stream`: no host synchronisation, no allocation (CUDA-graph capturable).  Errors: PCT_ERR_STATE before pct_reset;
+ * PCT_ERR_INVALID for n < 0, k < 1 or n * k > INT32_MAX.  n == 0: no-op.  The envs named in one call must be distinct (caller's
+ * contract, as for pct_restore).
+ *
+ * BoxCreator.preview(k) (D:binCreator.py:15-18), batched and read-only: d_out[i][0] = env d_env[i]'s CURRENT item (next_box,
+ * next_den); d_out[i][j >= 1] = the item its source delivers at draw draw_pos + j - 1 (d_env NULL: env i).  n x k x 4 float64
+ * [x, y, z, density]; the density is 1 outside setting 3, as the draws deliver it.  Every item mode: the random item set (setting 3
+ * densities included), continuous sample_from_distribution, and per-env streams, which wrap cyclically.  The preview lists raw
+ * consecutive draws: a reset in between (the jump to the next trajectory of pct_set_trajectory_length) makes the entries past it
+ * stale.  A row whose index is outside [0, n_envs) is all zeros. */
+int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, double *d_out, void *stream);
+
+/* env d_env[i] <- item i as its current item (d_env NULL: env i): `env.next_box = item; env.next_den = density` followed by the leaf
+ * expansion of cur_observation (D:bin3D.py:70-93, without gen_next_box), whose observation rows are written to d_obs (n_envs x obs_len,
+ * the layout and delta-row buffer contract of pct_step).
+ *   d_items  : n x 3 sizes, int32 (discrete; clamped to [0, 255], the range of a container side) / float64 (continuous)
+ *   d_density: n densities, or NULL = keep each env's current density (the draws deliver 1 outside setting 3)
+ *   d_info   : n_envs pct_step_info records (may be NULL): counter, sticky flags, n_leaf, n_cand, n_ems; ratio / ep_reward / ep_len 0.
+ * No draw is consumed (draw_pos is unchanged).  The set item stays the env's current item until a step places it or the env
+ * resets: the next step's reward, LeafNode2Action check and placement use it, a snapshot records it, and after a successful step
+ * the env continues with its source's next draw — as in the reference, where `env.next_box = X` then `step` pops the creator's head,
+ * not X (D:bin3D.py:180-182).  One difference: after a FAILED step with no_auto_reset the reference's terminal observation
+ * re-reads the creator's head (cur_observation -> gen_next_box = preview(1)[0]); here the env keeps the set item, so the terminal
+ * observation's item row and leaf rows are those of the set item (what pct_set_items wrote for it).
+ * Whole-batch re-expansion: EVERY env of the handle is re-expanded, not only the listed ones, and d_obs receives every env's rows.
+ * Envs not listed keep their item and come out bit-identical (same leaves, same rows: the shuffle keys depend on draw_pos only).  So
+ * the call costs about one pct_step minus its apply kernel, whatever n is; branch the envs to search over into a handle of their
+ * own (pct_snapshot / pct_restore) to pay for those alone.  Capacity flags raised by the new item's expansion are sticky as usual:
+ * reported in d_info and by the next step. */
+int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
+                  pct_step_info *d_info, void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

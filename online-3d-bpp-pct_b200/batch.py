@@ -306,6 +306,58 @@ class PctBatch(object):
                                            C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_height_maps")
         return out
 
+    # -- item preview and item override (include/pct_b200.h): lookahead and buffer packing ---------------------------------
+    def preview_items(self, k=1, env_idx=None, out=None):
+        """BoxCreator.preview(k) (binCreator.py) of envs env_idx (default: every env) -> (n, k, 4) float64 CUDA tensor of [x, y, z, density],
+        filled on the current stream (graph-capturable, read-only).  [:, 0] is each env's current item (preview_items()[:, 0, :3] is the
+        batched current-item accessor), [:, j] the item its source delivers j - 1 draws later.  A reset in between (trajectory jumps)
+        makes the entries past it stale.  Rows of an index outside [0, n_envs) are zeros."""
+        k = int(k)
+        if k < 1:
+            raise PctError("preview_items: k must be >= 1")
+        idx = self._index(env_idx, "env_idx")
+        n = self.n_envs if idx is None else int(idx.numel())
+        shape = (n, k, 4)
+        out = torch.empty(shape, dtype=torch.float64, device=self.device) if out is None else self._out(out, shape, torch.float64, "preview_items out")
+        self._check(self.L.pct_preview_items(self.h, C.c_void_p(idx.data_ptr()) if idx is not None and n else None, n, k,
+                                             C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_preview_items")
+        return out
+
+    def set_items(self, items, env_idx=None, density=None, out=None, info=None):
+        """Env env_idx[i] (default: env i) <- items[i] as its current item, without consuming a draw, then the leaf expansion of
+        cur_observation for it (the reference's `env.next_box = item` + get_possible_position()).  items: (n, 3) sizes, converted to int32
+        (discrete) / float64 (continuous); density: (n,) densities (default: keep each env's current density).  EVERY env of the batch is
+        re-expanded (envs not listed come out unchanged), and the complete observation goes to `out` (default: the batch's own observation
+        buffer, under the delta-row contract of step), which is returned.  info: optional (n_envs, 8) int32 tensor for the pct_step_info
+        records (capacity flags of the new expansions, n_leaf, ...).  The envs of one call must be distinct.  No items (n == 0): nothing is
+        enqueued and nothing is written."""
+        qd = torch.float64 if self.continuous else torch.int32
+        if not torch.is_tensor(items):
+            items = torch.as_tensor(np.asarray(items))
+        if items.dim() != 2 or items.shape[1] != 3:
+            raise PctError("items must have shape (n, 3): [x, y, z] per item")
+        n = int(items.shape[0])
+        it = items.to(device=self.device, dtype=qd).contiguous()
+        idx = self._index(env_idx, "env_idx")
+        if idx is not None and int(idx.numel()) != n:
+            raise PctError("env_idx must have one entry per item (%d)" % n)
+        if idx is None and n > self.n_envs:
+            raise PctError("%d items without env_idx for %d envs" % (n, self.n_envs))
+        den = None
+        if density is not None:
+            if not torch.is_tensor(density):
+                density = torch.as_tensor(np.asarray(density, dtype=np.float64))
+            if tuple(density.shape) != (n,):
+                raise PctError("density must have shape (n,) = (%d,)" % n)
+            den = density.to(device=self.device, dtype=torch.float64).contiguous()
+        obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "set_items out")
+        if info is not None:
+            info = self._out(info, (self.n_envs, 8), torch.int32, "set_items info")
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
+        self._check(self.L.pct_set_items(self.h, ptr(idx), n, ptr(it), ptr(den), C.c_void_p(obs.data_ptr()), ptr(info), self._stream()),
+                    "pct_set_items")
+        return obs
+
     # -- host-buffer API (what the reference's VecEnv exchanges over its pipes) --------------------------------
     def reset_host(self, obs_out):
         self._check(self.L.pct_reset_host(self.h, C.c_void_p(obs_out.ctypes.data)), "pct_reset_host")

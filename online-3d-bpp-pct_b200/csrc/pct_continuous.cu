@@ -1005,6 +1005,46 @@ __global__ void pctc_policy_random_kernel(const CEnv *env, int n_envs, int64_t e
     leaf_idx[e] = n > 0 ? (int32_t)(rnd_u64(seed, (uint64_t)(env_id_base + e), (uint64_t)t) % (uint64_t)n) : 0;
 }
 
+// ================= item preview / item override (pct_preview_items / pct_set_items; discrete twins and notes: pct_items.cu) =================
+__global__ void __launch_bounds__(256) pctc_preview_kernel(const CParams p, const ItemParams ip) {
+    const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (t >= (int64_t)ip.n * ip.k) return;
+    const int r = (int)(t / ip.k), j = (int)(t - (int64_t)r * ip.k);
+    const int e = ip.env ? ip.env[r] : r;
+    double *o = ip.out + (size_t)t * 4;
+    if (e < 0 || e >= p.n_envs) {  // not an env of this handle: a zero row
+        o[0] = 0; o[1] = 0; o[2] = 0; o[3] = 0;
+        return;
+    }
+    CHdr h = p.env[e].h;
+    if (j > 0) {
+        h.draw_pos += j - 1;
+        draw_item_c(p, e, h);
+    }
+    o[0] = h.next_box[0]; o[1] = h.next_box[1]; o[2] = h.next_box[2]; o[3] = h.next_den;
+}
+
+// stands in for pctc_apply_kernel: thread t writes item t (t < n) and initialises env t's info record (t < n_envs)
+__global__ void __launch_bounds__(256) pctc_set_items_kernel(const CParams p, const ItemParams ip) {
+    const int t = blockIdx.x * 256 + threadIdx.x;
+    if (t < ip.n) {
+        const int e = ip.env ? ip.env[t] : t;
+        if (e >= 0 && e < p.n_envs) {
+            const double *it = (const double *)ip.items + (size_t)t * 3;
+            CHdr &h = p.env[e].h;
+            h.next_box[0] = it[0]; h.next_box[1] = it[1]; h.next_box[2] = it[2];
+            if (ip.density) h.next_den = ip.density[t];
+        }
+    }
+    if (t < p.n_envs && p.info) {
+        const CHdr &h = p.env[t].h;
+        pct_step_info info{};
+        info.counter = h.n_box;
+        info.flags = h.flags;
+        p.info[t] = info;
+    }
+}
+
 // ================= host side =================
 int continuous_create(pct_env_batch *h) {
     cudaError_t e = cudaMalloc(&h->c_state, sizeof(CEnv) * (size_t)h->n_envs);
@@ -1027,8 +1067,28 @@ int continuous_create(pct_env_batch *h) {
 void continuous_destroy(pct_env_batch *h) { cudaFree(h->c_state); h->c_state = nullptr; cudaFree(h->c_walkq); h->c_walkq = nullptr; }
 int64_t continuous_state_bytes() { return (int64_t)sizeof(CEnv); }
 
+// CParams of the whole batch for the kernels that only read the item source (pct_preview_items)
+static CParams item_params(const pct_env_batch *h) {
+    CParams p{};
+    p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs; p.setting = h->cfg.setting;
+    p.item_mode = h->item_mode; p.sample_dist = h->cfg.sample_from_distribution;
+    p.sample_a = h->cfg.sample_left_bound; p.sample_b = h->cfg.sample_right_bound;
+    p.item_set = h->d_item_set; p.n_items = h->n_items; p.stream = h->d_stream; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
+    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base;
+    return p;
+}
+
+int continuous_preview(pct_env_batch *h, const ItemParams &ip, cudaStream_t st) {
+    const int64_t n = (int64_t)ip.n * ip.k;
+    pctc_preview_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(item_params(h), ip);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { h->err = std::string("pct_preview_items: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
+    return PCT_OK;
+}
+
+// set_items non-null (pct_set_items): pctc_set_items_kernel in place of the apply kernel, then the rest of the step's sequence in plain stream order
 int continuous_launch(pct_env_batch *h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
-                      uint8_t *done, pct_step_info *info, cudaStream_t st) {
+                      uint8_t *done, pct_step_info *info, cudaStream_t st, const ItemParams *set_items) {
     CParams p{};
     p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs;
     p.W = h->cfg.container_size[0]; p.L = h->cfg.container_size[1]; p.H = h->cfg.container_size[2];
@@ -1043,10 +1103,13 @@ int continuous_launch(pct_env_batch *h, int mode, const void *actions, int actio
     p.mode = mode; p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(st, &cap);
-    if (h->overlap_cont && h->d_ready && cap == cudaStreamCaptureStatusNone) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
+    if (h->overlap_cont && h->d_ready && cap == cudaStreamCaptureStatusNone && !set_items) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
     const bool stab = p.setting != 2;
     const int b2 = (p.n_envs + 1) / 2;
-    if (stab && h->alias_mode && h->d_aux) {
+    if (set_items) {
+        const int n = max(set_items->n, p.n_envs);
+        pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, *set_items);
+    } else if (stab && h->alias_mode && h->d_aux) {
         p.aux = h->d_aux;
         pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);
     } else if (stab) pctc_apply_kernel<true><<<b2, 64, 0, st>>>(p);

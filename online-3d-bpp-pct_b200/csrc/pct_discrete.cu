@@ -540,23 +540,9 @@ __device__ __noinline__ int gen_level_points(const int16_t (*box)[6], int n_box,
     return n;
 }
 
-// ---- item source ------------------------------------------------------------------------------------------
-__device__ __noinline__ void draw_item(const DParams &p, int e, DHdr &h) {
-    const uint64_t gid = (uint64_t)(p.env_id_base + e);
-    const uint64_t d = (uint64_t)h.draw_pos;
-    const double *it;
-    if (p.item_mode == 0) {
-        it = p.item_set + (rnd_u64(p.seed, gid, d) % (uint64_t)p.n_items) * 3;
-        h.next_den = p.setting == 3 ? rnd_density(p.seed, gid, d) : 1.0;
-    } else {
-        it = p.stream + ((size_t)e * p.stream_len + (size_t)(d % (uint64_t)p.stream_len)) * 4;
-        h.next_den = p.setting == 3 ? it[3] : 1.0;
-    }
-    h.next_box[0] = (int)it[0];
-    h.next_box[1] = (int)it[1];
-    h.next_box[2] = (int)it[2];
-    h.draw_pos++;
-}
+}  // namespace pct
+#include "pct_draw.cuh"  // the item source, draw_item (included here, between the phases it sits among in the code layout)
+namespace pct {
 
 // Space.reset (D:space.py:290-314) + box_creator.reset / generate_box_size (D:bin3D.py:62-65)
 __device__ __noinline__ void reset_space(DEnvHot *hot, const DParams &p, int e, int lane) {
@@ -1510,8 +1496,9 @@ static cudaError_t set_smem(K kernel, size_t smem) {
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 }
 
+// apply = false: the pipeline without K1 (pct_set_items: pct_set_items_kernel has already written the items); the caller passes ready = order = nullptr
 template <typename OT, bool STAB, typename SlotT>
-static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *prof) {
+static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
     constexpr bool BIGSM = !STAB;
     static bool attr_set = false;
     static int n_sm = 0;
@@ -1532,8 +1519,10 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
     }
     const int blocks = (p.n_envs + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
     if (prof) cudaEventRecord(prof[0], st);
-    if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
-    else pct_apply_kernel<STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+    if (apply) {
+        if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+        else pct_apply_kernel<STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+    }
     if (prof) cudaEventRecord(prof[1], st);
     cudaError_t err = cudaSuccess;
     if (p.ready) {
@@ -1585,9 +1574,9 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
     return cudaGetLastError();
 }
 template <typename OT, bool STAB>
-static cudaError_t launch_s(const DParams &p, cudaStream_t st, cudaEvent_t *prof) {
-    if (p.W <= 16 && p.L <= 16 && p.H <= 16) return launch_t<OT, STAB, uint16_t>(p, st, prof);
-    return launch_t<OT, STAB, uint32_t>(p, st, prof);
+static cudaError_t launch_s(const DParams &p, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
+    if (p.W <= 16 && p.L <= 16 && p.H <= 16) return launch_t<OT, STAB, uint16_t>(p, st, prof, apply);
+    return launch_t<OT, STAB, uint32_t>(p, st, prof, apply);
 }
 
 // number of kernels one reset / step enqueues (for pct_kernel_launches): apply, candidates (+ classify), [walk], emit, order / pool reset
@@ -1596,10 +1585,10 @@ int discrete_kernels_per_step(const DParams &p) {
     return 3 + (p.setting != 2 ? 2 : 0);
 }
 
-cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof) {
+cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof, bool apply) {
     const bool stab = p.setting != 2;
-    if (p.obs_f64) return stab ? launch_s<double, true>(p, st, prof) : launch_s<double, false>(p, st, prof);
-    return stab ? launch_s<float, true>(p, st, prof) : launch_s<float, false>(p, st, prof);
+    if (p.obs_f64) return stab ? launch_s<double, true>(p, st, prof, apply) : launch_s<double, false>(p, st, prof, apply);
+    return stab ? launch_s<float, true>(p, st, prof, apply) : launch_s<float, false>(p, st, prof, apply);
 }
 
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,

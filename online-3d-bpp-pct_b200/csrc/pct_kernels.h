@@ -268,11 +268,24 @@ cudaError_t launch_queries_discrete(const DParams &p, const QParams &q, cudaStre
 // Space.plain[:W, :L] of envs env[0..n) (nullptr: 0..n-1) -> out, n x W x L int32
 cudaError_t launch_height_maps(const DParams &p, const int32_t *env, int n, int32_t *out, cudaStream_t st);
 
+// item preview / item override (pct_items.cu; continuous: pct_continuous.cu)
+struct ItemParams {
+    const int32_t *env;      // [n] env of row / item i, nullptr: env i
+    int n, k;                // rows; preview: items per row
+    const void *items;       // set: n x 3 sizes, int32 (discrete) / float64 (continuous)
+    const double *density;   // set: n densities, nullptr: keep each env's current density
+    double *out;             // preview: n x k x 4 [x, y, z, density]
+};
+cudaError_t launch_preview_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
+// the item kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
+cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
+
 // delta observation writes: aux[i].obs_prev = {nb, nl} for n envs ("every row of the buffer may be non-zero")
 void launch_fill_prev(DEnvAux *aux, int n_envs, int nb, int nl, cudaStream_t st);
 
 int discrete_kernels_per_step(const DParams &p);
-cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof = nullptr);
+// apply = false: the sequence without the apply kernel (pct_set_items; p.ready and p.order must be nullptr)
+cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof = nullptr, bool apply = true);
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                           cudaStream_t st, const int64_t *t_dev = nullptr);
 
