@@ -250,6 +250,30 @@ int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, 
 int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
                   pct_step_info *d_info, void *stream);
 
+/* env.reset() (D:bin3D.py:61-67, C:bin3D.py:69-75) for chosen envs of the batch: start new episodes in some envs and leave the others
+ * as they are.  For gym semantics on a whole batch (no_auto_reset = 1: the caller sees the terminal observation, then resets the
+ * finished envs), episode control under auto-reset (time limits, curricula, dropping an episode), and device-resident loops, where a
+ * captured graph resets on the step's own done bytes (policy -> pct_step -> pct_reset_envs(d_mask = d_done)).
+ * Exactly one of d_env / d_mask is non-NULL:
+ *   d_env : n env indices.  They must be distinct (caller's contract, as for pct_restore); an index outside [0, n_envs) is skipped.
+ *   d_mask: n_envs bytes, n == n_envs; env e resets iff d_mask[e] != 0.  The d_done buffer of the preceding pct_step can be passed as is.
+ * A selected env gets exactly what pct_step's auto-reset does to a finished env: counters, sticky flags, the EMS list, boxes and loads
+ * are cleared; the draw position is kept (under pct_set_trajectory_length it jumps to the start of the next trajectory,
+ * LoadBoxCreator.reset) and a fresh item is drawn.  The current item is discarded, as RandomBoxCreator.reset() discards its list,
+ * including an item set by pct_set_items.  An env's items depend on its global id only, so sharding does not change them.  Resets in
+ * mid-episode are allowed, with or without no_auto_reset.
+ *   d_obs : n_envs x obs_len, every env's observation rows, under the layout and delta-row buffer contract of pct_step
+ *   d_info: n_envs pct_step_info records (may be NULL), as pct_set_items writes them: counter, sticky flags, n_leaf, n_cand, n_ems;
+ *           ratio / ep_reward / ep_len 0.  (The terminal records are the ones the preceding pct_step wrote.)
+ * Enqueue only: no host synchronisation, no allocation (CUDA-graph capturable).  n == 0 (d_env): no-op.  Errors: PCT_ERR_STATE before
+ * pct_reset; PCT_ERR_INVALID when both or neither of d_env / d_mask are given, for n < 0, and for a mask with n != n_envs.
+ * Whole-batch re-expansion, as for pct_set_items: EVERY env of the handle is re-expanded and gets its rows written to d_obs; envs not
+ * selected come out bit-identical.  So the call costs about one pct_step minus its apply kernel however few envs it resets, an
+ * all-zero mask included (less when many envs reset: empty bins expand fast).  A caller of the gym loop who keeps the terminal
+ * observations must copy them out of d_obs first (the reset overwrites the rows of the reset envs); passing the reset another buffer
+ * than the step's forces full row writes. */
+int pct_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

@@ -43,7 +43,7 @@ EXPORTS = ["pct_create", "pct_destroy", "pct_last_error", "pct_set_item_set", "p
            "pct_state_bytes_per_env", "pct_kernel_launches", "pct_version", "pct_profile_enable", "pct_profile_read", "pct_heuristic_actions",
            "pct_heuristic_actions_f64", "pct_query_placement", "pct_query_placement_f64",
            "pct_snapshot_bytes", "pct_snapshot", "pct_restore", "pct_query_placements", "pct_query_placements_f64", "pct_height_maps",
-           "pct_preview_items", "pct_set_items"]
+           "pct_preview_items", "pct_set_items", "pct_reset_envs"]
 
 
 def build(verbose=False):
@@ -102,5 +102,6 @@ def lib():
     L.pct_height_maps.argtypes = [vp, vp, i32, vp, vp]
     L.pct_preview_items.argtypes = [vp, vp, i32, i32, vp, vp]
     L.pct_set_items.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
+    L.pct_reset_envs.argtypes = [vp, vp, i32, vp, vp, vp, vp]
     _lib = L
     return L

@@ -109,10 +109,46 @@ class PctBatch(object):
         self._check(self.L.pct_set_trajectory_length(self.h, int(traj_len)), "pct_set_trajectory_length")
 
     # -- device-resident API -------------------------------------------------------------------------------
-    def reset(self, out=None):
-        obs = self._obs if out is None else out
-        self._check(self.L.pct_reset(self.h, C.c_void_p(obs.data_ptr()), self._stream()), "pct_reset")
-        self.did_reset = True
+    def reset(self, out=None, env_idx=None, mask=None, info=None):
+        """Without env_idx / mask: reset every env (VecEnv.reset()).  With one of them: env.reset() for the chosen envs only
+        (pct_reset_envs, include/pct_b200.h), enqueued on the current stream (graph-capturable) after a first full reset.  env_idx: distinct
+        env indices (indices outside [0, n_envs) are skipped); mask: an (n_envs,) bool / uint8 tensor, e.g. the `done` of the last step,
+        so `reset(mask=done)` gives gym semantics to a batch built with auto_reset=False.  Every env of the batch is re-expanded (envs not
+        chosen come out unchanged) and the complete observation goes to `out` (default: the batch's own observation buffer, under the
+        delta-row contract of step), which is returned: clone() a terminal observation before resetting over it.  info: optional
+        (n_envs, 8) int32 tensor for the pct_step_info records of the new expansions.  An empty env_idx enqueues nothing."""
+        if env_idx is None and mask is None:
+            if info is not None:
+                raise PctError("reset: info is written by a reset of chosen envs (env_idx or mask) only")
+            obs = self._obs if out is None else out
+            self._check(self.L.pct_reset(self.h, C.c_void_p(obs.data_ptr()), self._stream()), "pct_reset")
+            self.did_reset = True
+            return obs
+        if env_idx is not None and mask is not None:
+            raise PctError("reset: pass env_idx or mask, not both")
+        if not self.did_reset:
+            raise PctError("reset(env_idx / mask) before the first reset() of the batch")
+        obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "reset out")
+        if info is not None:
+            info = self._out(info, (self.n_envs, 8), torch.int32, "reset info")
+        idx = m = None
+        if mask is not None:
+            if not torch.is_tensor(mask):
+                mask = torch.as_tensor(np.asarray(mask))
+            if mask.dtype not in (torch.bool, torch.uint8) or tuple(mask.shape) != (self.n_envs,):
+                raise PctError("reset mask must be an (n_envs,) = (%d,) bool or uint8 tensor" % self.n_envs)
+            m = mask.to(self.device).contiguous()
+            if m.dtype == torch.bool:
+                m = m.view(torch.uint8)  # same bytes (0 / 1): no copy, so a captured graph reads the caller's tensor
+            n = self.n_envs
+        else:
+            idx = self._index(env_idx, "env_idx")
+            n = int(idx.numel())
+            if n == 0:
+                return obs
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        self._check(self.L.pct_reset_envs(self.h, ptr(idx), n, ptr(m), C.c_void_p(obs.data_ptr()), ptr(info), self._stream()),
+                    "pct_reset_envs")
         return obs
 
     def step(self, actions=None, leaf_idx=None, out=None):

@@ -28,7 +28,7 @@ namespace pct {
 int continuous_create(pct_env_batch *h);
 void continuous_destroy(pct_env_batch *h);
 int continuous_launch(pct_env_batch *h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
-                      uint8_t *done, pct_step_info *info, cudaStream_t st, const ItemParams *set_items = nullptr);
+                      uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre = nullptr);
 int continuous_preview(pct_env_batch *h, const ItemParams &ip, cudaStream_t st);
 int continuous_policy_random(pct_env_batch *h, int32_t *leaf_idx, uint64_t seed, int64_t t, cudaStream_t st);
 int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out);
@@ -246,9 +246,9 @@ static void begin_obs(pct_handle h, const void *obs) {
     h->tracked_obs = obs;
 }
 
-// set_items non-null (pct_set_items): the item kernel replaces the apply kernel; whole batch, non-overlapped order, env order (no LPT parity flip)
+// pre non-null (pct_set_items / pct_reset_envs): its kernel replaces the apply kernel; whole batch, non-overlapped order, env order (no LPT parity flip)
 static int launch_range(pct_handle h, int mode, int off, int cnt, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs,
-                        float *rew, uint8_t *done, pct_step_info *info, cudaStream_t gs, bool whole_batch, const ItemParams *set_items = nullptr) {
+                        float *rew, uint8_t *done, pct_step_info *info, cudaStream_t gs, bool whole_batch, const PreKernel *pre = nullptr) {
     const size_t osz = h->cfg.obs_dtype == PCT_F64 ? 8 : 4, asz = action_f64 ? 8 : 4;
     DParams p{};
     p.hot = h->d_hot + off; p.cold = h->d_cold + off; p.n_envs = cnt;
@@ -263,13 +263,13 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
     p.obs = (char *)obs + (size_t)off * h->obs_len * osz; p.obs_f64 = h->cfg.obs_dtype == PCT_F64;
     p.reward = rew ? rew + off : nullptr; p.done = done ? done + off : nullptr; p.info = info ? info + off : nullptr; p.mode = mode;
     p.dbg = (long long *)h->dbg;
-    p.order = (h->lpt && whole_batch && !set_items) ? h->d_order : nullptr;
+    p.order = (h->lpt && whole_batch && !pre) ? h->d_order : nullptr;
     p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
     // overlapped launch mode: not while a CUDA graph is being captured (the epoch would be frozen into the graph and a replay
     // would find the flags of the previous replay already set), not under the per-kernel profiler, not with the LPT permutation
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(gs, &cap);
-    if (h->overlap && !h->prof_on && cap == cudaStreamCaptureStatusNone && !set_items) {
+    if (h->overlap && !h->prof_on && cap == cudaStreamCaptureStatusNone && !pre) {
         p.ready = h->d_ready + 2 * (size_t)off;
         p.epoch = ++h->epoch;
     }
@@ -281,7 +281,7 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
     if (h->k3_block) p.opt |= PCT_OPT_K3_BLOCK;
     if (h->no_emit_pdl) p.opt |= PCT_OPT_NO_EMIT_PDL;
     cudaEvent_t *prof = nullptr;
-    if (h->prof_on && mode == 1 && whole_batch && !set_items) {
+    if (h->prof_on && mode == 1 && whole_batch && !pre) {
         if ((size_t)(h->prof_steps + 1) * 4 > h->prof_ev.size()) {
             const size_t old = h->prof_ev.size();
             h->prof_ev.resize(old + 4096, nullptr);
@@ -298,7 +298,7 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
     p.walk_fork = h->walk_fork ? 1 : 0; p.walk_blocks = h->walk_blocks; p.walk_keep = h->walk_keep; p.piece_cap = cnt * WALK_PIECES_PER_ENV;
     p.piece_ready = h->d_piece_ready ? h->d_piece_ready + (size_t)off * WALK_PIECES_PER_ENV : nullptr;
     p.walk_pend = h->d_walk_pend ? h->d_walk_pend + (size_t)off * CAND_MAX : nullptr;
-    if (set_items) CK(h, launch_set_items_discrete(p, *set_items, gs));
+    if (pre) CK(h, pre->items ? launch_set_items_discrete(p, *pre->items, gs) : launch_reset_envs_discrete(p, *pre->reset, gs));
     else CK(h, launch_discrete(p, gs, prof));
     h->launches += discrete_kernels_per_step(p);
     return PCT_OK;
@@ -651,24 +651,41 @@ int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, 
     return PCT_OK;
 }
 
+// pct_set_items / pct_reset_envs: the pre-kernel in place of the apply kernel, then the rest of the step's pipeline over the whole batch,
+// on the caller's stream whatever PCT_B200_GROUPS says
+static int launch_pre(pct_handle h, const PreKernel &pre, void *d_obs, pct_step_info *d_info, cudaStream_t st) {
+    CK(h, cudaSetDevice(h->device));
+    begin_obs(h, d_obs);
+    if (h->cfg.domain == PCT_CONTINUOUS) {
+        const int rc = continuous_launch(h, 1, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, &pre);
+        if (rc == PCT_OK) h->launches++;
+        return rc;
+    }
+    const int rc = launch_range(h, 1, 0, h->n_envs, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, true, &pre);
+    h->fill_pending = false;
+    return rc;
+}
+
 int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
                   pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
     int rc = check_items(h, "pct_set_items", n, 1, d_items, "d_items");
     if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs) { h->err = "pct_set_items: d_obs is NULL"; return PCT_ERR_INVALID; }
-    CK(h, cudaSetDevice(h->device));
-    begin_obs(h, d_obs);
     const ItemParams ip{d_env, n, 1, d_items, d_density, nullptr};
-    cudaStream_t st = (cudaStream_t)stream;
-    if (h->cfg.domain == PCT_CONTINUOUS) {
-        rc = continuous_launch(h, 1, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, &ip);
-        if (rc == PCT_OK) h->launches++;
-        return rc;
-    }
-    rc = launch_range(h, 1, 0, h->n_envs, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, true, &ip);
-    h->fill_pending = false;
-    return rc;
+    return launch_pre(h, PreKernel{&ip, nullptr}, d_obs, d_info, (cudaStream_t)stream);
+}
+
+int pct_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    if ((d_env == nullptr) == (d_mask == nullptr)) { h->err = "pct_reset_envs: pass exactly one of d_env / d_mask"; return PCT_ERR_INVALID; }
+    if (n < 0) { h->err = "pct_reset_envs: n must be >= 0"; return PCT_ERR_INVALID; }
+    if (d_mask && n != h->n_envs) { h->err = "pct_reset_envs: a mask has n_envs entries (n = " + std::to_string(n) + ")"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_reset_envs before pct_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    if (!d_obs) { h->err = "pct_reset_envs: d_obs is NULL"; return PCT_ERR_INVALID; }
+    const ResetParams rp{d_env, n, d_mask};
+    return launch_pre(h, PreKernel{nullptr, &rp}, d_obs, d_info, (cudaStream_t)stream);
 }
 
 int pct_get_state(pct_handle h, int32_t env, pct_state_dump *out) {

@@ -1005,7 +1005,7 @@ __global__ void pctc_policy_random_kernel(const CEnv *env, int n_envs, int64_t e
     leaf_idx[e] = n > 0 ? (int32_t)(rnd_u64(seed, (uint64_t)(env_id_base + e), (uint64_t)t) % (uint64_t)n) : 0;
 }
 
-// ================= item preview / item override (pct_preview_items / pct_set_items; discrete twins and notes: pct_items.cu) =================
+// ================= item preview / item override / per-env reset (pct_preview_items / pct_set_items / pct_reset_envs; discrete twins and notes: pct_items.cu) =================
 __global__ void __launch_bounds__(256) pctc_preview_kernel(const CParams p, const ItemParams ip) {
     const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
     if (t >= (int64_t)ip.n * ip.k) return;
@@ -1042,6 +1042,23 @@ __global__ void __launch_bounds__(256) pctc_set_items_kernel(const CParams p, co
         info.counter = h.n_box;
         info.flags = h.flags;
         p.info[t] = info;
+    }
+}
+
+// stands in for pctc_apply_kernel (pct_reset_envs): warp w resets env w with reset_space_c if selected, then writes its info record
+__global__ void __launch_bounds__(256) pctc_reset_envs_kernel(const CParams p, const ResetParams rp) {
+    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (e >= p.n_envs) return;  // the whole warp
+    bool sel = rp.mask && rp.mask[e] != 0;
+    if (!rp.mask)
+        for (int i0 = 0; i0 < rp.n && !sel; i0 += 32) sel = __any_sync(FULL, i0 + lane < rp.n && rp.env[i0 + lane] == e);
+    CEnv *ev = p.env + e;
+    if (sel) reset_space_c(ev, p, e, lane);
+    if (lane == 0 && p.info) {
+        pct_step_info info{};
+        info.counter = ev->h.n_box;
+        info.flags = ev->h.flags;
+        p.info[e] = info;
     }
 }
 
@@ -1086,9 +1103,9 @@ int continuous_preview(pct_env_batch *h, const ItemParams &ip, cudaStream_t st) 
     return PCT_OK;
 }
 
-// set_items non-null (pct_set_items): pctc_set_items_kernel in place of the apply kernel, then the rest of the step's sequence in plain stream order
+// pre non-null (pct_set_items / pct_reset_envs): its kernel in place of the apply kernel, then the rest of the step's sequence in plain stream order
 int continuous_launch(pct_env_batch *h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
-                      uint8_t *done, pct_step_info *info, cudaStream_t st, const ItemParams *set_items) {
+                      uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre) {
     CParams p{};
     p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs;
     p.W = h->cfg.container_size[0]; p.L = h->cfg.container_size[1]; p.H = h->cfg.container_size[2];
@@ -1103,12 +1120,14 @@ int continuous_launch(pct_env_batch *h, int mode, const void *actions, int actio
     p.mode = mode; p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(st, &cap);
-    if (h->overlap_cont && h->d_ready && cap == cudaStreamCaptureStatusNone && !set_items) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
+    if (h->overlap_cont && h->d_ready && cap == cudaStreamCaptureStatusNone && !pre) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
     const bool stab = p.setting != 2;
     const int b2 = (p.n_envs + 1) / 2;
-    if (set_items) {
-        const int n = max(set_items->n, p.n_envs);
-        pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, *set_items);
+    if (pre && pre->items) {
+        const int n = max(pre->items->n, p.n_envs);
+        pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, *pre->items);
+    } else if (pre) {
+        pctc_reset_envs_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, *pre->reset);
     } else if (stab && h->alias_mode && h->d_aux) {
         p.aux = h->d_aux;
         pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);

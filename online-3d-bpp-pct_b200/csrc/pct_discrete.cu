@@ -541,21 +541,8 @@ __device__ __noinline__ int gen_level_points(const int16_t (*box)[6], int n_box,
 }
 
 }  // namespace pct
-#include "pct_draw.cuh"  // the item source, draw_item (included here, between the phases it sits among in the code layout)
+#include "pct_draw.cuh"  // the item source and the env reset, draw_item / reset_space (included here, between the phases they sit among in the code layout)
 namespace pct {
-
-// Space.reset (D:space.py:290-314) + box_creator.reset / generate_box_size (D:bin3D.py:62-65)
-__device__ __noinline__ void reset_space(DEnvHot *hot, const DParams &p, int e, int lane) {
-    if (lane == 0) {
-        DHdr &h = hot->h;
-        h.n_box = 0; h.n_ems = 1; h.n_leaf = 0; h.flags = 0; h.n_edge = 0; h.n_poly = 0; h.vol_sum = 0; h.ep_len = 0; h.ep_reward = 0;
-        hot->ems[0][0] = 0; hot->ems[0][1] = 0; hot->ems[0][2] = 0;
-        hot->ems[0][3] = (int16_t)p.W; hot->ems[0][4] = (int16_t)p.L; hot->ems[0][5] = (int16_t)p.H;
-        if (p.traj_len > 0 && h.draw_pos % p.traj_len) h.draw_pos += p.traj_len - h.draw_pos % p.traj_len;  // LoadBoxCreator.reset
-        draw_item(p, e, h);
-    }
-    __syncwarp();
-}
 
 // Delta variant (default, PCT_B200_OBS_DELTA=0 disables): the caller hands back the SAME observation buffer every step, and prev[0] / prev[1]
 // hold how many internal / leaf rows of it may be non-zero.  75 % of the (NB + NL + 1) x 9 observation is zero padding, so only the
@@ -1496,7 +1483,7 @@ static cudaError_t set_smem(K kernel, size_t smem) {
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 }
 
-// apply = false: the pipeline without K1 (pct_set_items: pct_set_items_kernel has already written the items); the caller passes ready = order = nullptr
+// apply = false: the pipeline without K1 (pct_set_items / pct_reset_envs: their kernel in pct_items.cu has already run); the caller passes ready = order = nullptr
 template <typename OT, bool STAB, typename SlotT>
 static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
     constexpr bool BIGSM = !STAB;

@@ -1,6 +1,8 @@
-// The item source of the discrete env: draw_item delivers the item of draw h.draw_pos and advances it.  The one place the item formulas live:
-// the step kernels (pct_discrete.cu) and the item preview (pct_items.cu) both include it.  The preview is a translation unit of its own because a
-// new caller inside pct_discrete.cu changed the register allocation of the apply kernels around their calls; `inline` lets both units define it.
+// The item source of the discrete env and the env reset that draws from it.  draw_item delivers the item of draw h.draw_pos and advances it;
+// reset_space is what a reset does to an env (the auto-reset of the apply kernel and the per-env reset of pct_reset_envs).  The one place
+// both live: the step kernels (pct_discrete.cu) and the item / reset kernels (pct_items.cu) include it.  Those kernels are a translation unit
+// of their own because a new caller inside pct_discrete.cu changed the register allocation of the apply kernels around their calls; `inline`
+// lets both units define the functions.
 #pragma once
 #include "pct_common.cuh"
 #include "pct_kernels.h"
@@ -22,6 +24,19 @@ __device__ __noinline__ inline void draw_item(const DParams &p, int e, DHdr &h) 
     h.next_box[1] = (int)it[1];
     h.next_box[2] = (int)it[2];
     h.draw_pos++;
+}
+
+// Space.reset (D:space.py:290-314) + box_creator.reset / generate_box_size (D:bin3D.py:62-65)
+__device__ __noinline__ inline void reset_space(DEnvHot *hot, const DParams &p, int e, int lane) {
+    if (lane == 0) {
+        DHdr &h = hot->h;
+        h.n_box = 0; h.n_ems = 1; h.n_leaf = 0; h.flags = 0; h.n_edge = 0; h.n_poly = 0; h.vol_sum = 0; h.ep_len = 0; h.ep_reward = 0;
+        hot->ems[0][0] = 0; hot->ems[0][1] = 0; hot->ems[0][2] = 0;
+        hot->ems[0][3] = (int16_t)p.W; hot->ems[0][4] = (int16_t)p.L; hot->ems[0][5] = (int16_t)p.H;
+        if (p.traj_len > 0 && h.draw_pos % p.traj_len) h.draw_pos += p.traj_len - h.draw_pos % p.traj_len;  // LoadBoxCreator.reset
+        draw_item(p, e, h);
+    }
+    __syncwarp();
 }
 
 }  // namespace pct

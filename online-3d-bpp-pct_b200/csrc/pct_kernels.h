@@ -280,11 +280,27 @@ cudaError_t launch_preview_discrete(const DParams &p, const ItemParams &ip, cuda
 // the item kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
 cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
 
+// per-env reset (pct_reset.cu; continuous: pct_continuous.cu): env e resets iff mask[e] != 0 (mask non-null) or e is one of env[0..n)
+struct ResetParams {
+    const int32_t *env;
+    int n;
+    const uint8_t *mask;     // [n_envs], or nullptr: the env list
+};
+// the reset kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
+cudaError_t launch_reset_envs_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st);
+
+// the kernel that stands in for the apply kernel of a step, exactly one non-null: the item kernel (pct_set_items) or the reset kernel
+// (pct_reset_envs).  The rest of the step's pipeline then re-expands every env of the batch.
+struct PreKernel {
+    const ItemParams *items;
+    const ResetParams *reset;
+};
+
 // delta observation writes: aux[i].obs_prev = {nb, nl} for n envs ("every row of the buffer may be non-zero")
 void launch_fill_prev(DEnvAux *aux, int n_envs, int nb, int nl, cudaStream_t st);
 
 int discrete_kernels_per_step(const DParams &p);
-// apply = false: the sequence without the apply kernel (pct_set_items; p.ready and p.order must be nullptr)
+// apply = false: the sequence without the apply kernel (pct_set_items / pct_reset_envs; p.ready and p.order must be nullptr)
 cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof = nullptr, bool apply = true);
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                           cudaStream_t st, const int64_t *t_dev = nullptr);
