@@ -171,8 +171,9 @@ int pct_policy_random_dev(pct_handle h, int32_t *d_leaf_idx, uint64_t seed, cons
  * placement (the reference then ends the episode without stepping, e.g. heuristic.py:223-225) the row is
  * [1,0,0,1,0,0,0,0,1], which no item matches, so pct_step ends the episode (PCT_FLAG_BAD_ACTION is set in its info).
  * Replaces the per-env Python loops over Space.drop_box_virtual (D:space.py:393-433).  LSAH keeps its running footprint
- * per env inside the handle.  PCT_H_RANDOM draws with rnd(seed, env_id_base+e, t).  PCT_H_BR needs pct_set_item_set;
- * PCT_H_HM / PCT_H_MACS / PCT_H_RANDOM need container sides <= 32. */
+ * per env inside the handle.  PCT_H_RANDOM draws with rnd(seed, env_id_base+e, t).  PCT_H_BR needs pct_set_item_set.
+ * Every baseline runs on every discrete container pct_create accepts (sides up to 255); PCT_H_RANDOM chooses among all
+ * feasible grid placements at any size.  The call only enqueues one kernel, so it can be captured in a CUDA graph. */
 int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64_t seed, int64_t t, void *stream);
 /* Same for the CONTINUOUS domain, where tools.py:217-218 allows PCT_H_LSAH, PCT_H_ONLINEBPH and PCT_H_BR only (heuristic.py
  * LASH :138-226, OnlineBPH :364-424, BR :500-577 over pct_envs.PctContinuous0): float64 rows (N x 9) for
@@ -183,7 +184,8 @@ int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64
 int pct_heuristic_actions_f64(pct_handle h, int32_t heuristic, double *d_rows, void *stream);
 /* Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH / returnMap) for ONE env (D:space.py:393-433): what
  * the reference's heuristic.py calls on `env.space`; synchronous.  height_map: W*L int32 (row-major, after the virtual
- * placement — Space.update_height_graph on a copy) or NULL. */
+ * placement — Space.update_height_graph on a copy) or NULL.  Container sides <= 32 (PCT_ERR_INVALID otherwise): for larger
+ * bins, pct_query_placements and pct_height_maps answer the same questions without a size limit. */
 int pct_query_placement(pct_handle h, int32_t env, const int32_t dims[3], int32_t lx, int32_t ly, double density,
                         int32_t *feasible, int32_t *rest_height, int32_t *height_map);
 

@@ -145,6 +145,9 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
             if (e == cudaSuccess) e = cudaMalloc(&h->d_ready, sizeof(int32_t) * 2 * (size_t)n_envs);
             if (e == cudaSuccess) e = cudaMemset(h->d_ready, 0, sizeof(int32_t) * 2 * (size_t)n_envs);
             if (e == cudaSuccess) e = cudaMemset(h->d_cold, 0, sizeof(DEnvCold) * (size_t)n_envs);
+            // HM / MACS / RANDOM on a bin wider than 32 cells run with dynamic shared memory: raise its limit here, so that
+            // pct_heuristic_actions stays enqueue-only (capturable)
+            if (e == cudaSuccess && (cfg->container_size[0] > HEUR_SIDE_MAX || cfg->container_size[1] > HEUR_SIDE_MAX)) e = prepare_heuristic_big();
             if (e == cudaSuccess && !h->k3_block) {  // the step's pool of stability walks: worst-case capacity, only the used prefix is ever touched
                 e = cudaMalloc(&h->d_walkq, sizeof(WalkItem) * (size_t)CAND_MAX * (size_t)n_envs);
                 if (e == cudaSuccess) e = cudaMalloc(&h->d_walk_ctr, sizeof(int32_t) * (size_t)n_envs);
@@ -500,10 +503,6 @@ int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64
     CK(h, cudaSetDevice(h->device));
     DParams p = state_params(h);
     if (heuristic == PCT_H_BR && !h->d_item_set) { h->err = "PCT_H_BR scores an EMS by the item types that fit: call pct_set_item_set"; return PCT_ERR_STATE; }
-    if ((heuristic == PCT_H_HM || heuristic == PCT_H_MACS || heuristic == PCT_H_RANDOM) && (p.W > HEUR_SIDE_MAX || p.L > HEUR_SIDE_MAX)) {
-        h->err = "PCT_H_HM / PCT_H_MACS / PCT_H_RANDOM need container sides <= 32";
-        return PCT_ERR_INVALID;
-    }
     HParams hp{};
     hp.code = heuristic; hp.rows = d_rows; hp.hstate = h->d_hstate; hp.seed = seed; hp.t = t;
     CK(h, launch_heuristic_discrete(p, hp, (cudaStream_t)stream));

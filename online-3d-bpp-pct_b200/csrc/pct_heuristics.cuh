@@ -17,6 +17,16 @@ namespace pct {
 constexpr int HM_CELLS_MAX = 1024;   // height map staged in shared memory (HM, MACS, placement queries): W * L <= 1024
 constexpr int HC_MAX = 6144;         // RANDOM: feasibility bitmap capacity (grid x rotations)
 
+// Large-container instantiation (BIG = true: HM, MACS and RANDOM when W or L > 32).  The height map, the RANDOM bitmap and MACS's
+// histogram rows then live in dynamic shared memory sized from W * L: the int16 map (padded to 16 bytes), then either the bitmap
+// (one bit per grid candidate, ceil(W * L * R / 32) words) or the histogram rows (byte j of thread t at j * FEAS_THREADS + t); only
+// one of the two is used by a launch.  At 255 x 255, R = 6 this is 130064 + 48768 bytes next to the static staging.
+__host__ __device__ constexpr size_t heur_big_map_bytes(int W, int L) { return ((size_t)W * L * 2 + 15) / 16 * 16; }
+__host__ __device__ constexpr size_t heur_big_smem(int W, int L, int R) {
+    const size_t bitmap = ((size_t)W * L * R + 31) / 32 * 4, rows = (size_t)FEAS_THREADS * L;
+    return heur_big_map_bytes(W, L) + (bitmap > rows ? bitmap : rows);
+}
+
 
 // `x, y, z = next_box`, `y, x, z = ...`, `z, x, y = ...`, `z, y, x = ...`, `x, z, y = ...`, `y, z, x = ...` (heuristic.py:176-187):
 // which entry of next_box becomes x / y / z.  (Not the EMSPoint rotation table.)
@@ -84,25 +94,30 @@ __device__ __forceinline__ HCand heur_decode(int code, int c, const int16_t (*em
 // calc_maximal_usable_spaces (heuristic.py:12-45) of the container after the placement, summed over the levels below
 // the rest height.  The reference tracks a voxel grid (boxes and the space under them are non-zero, :47-52); a voxel
 // (i, j, k) of it is non-zero exactly when k < height map(i, j), so "free at level k" is `height map after <= k`.
+// BIG: the row is this thread's column of the histogram rows in dynamic shared memory (values <= W <= 255 fit a byte).
+template <bool BIG>
 __device__ __noinline__ long long macs_score(const int16_t *hm, int W, int L, const HCand &k, int mh) {
     long long score = 0;
     const int top = mh + k.sz;
     for (int lev = 0; lev < mh; lev++) {
-        uint8_t hist[32];  // histogram row i: free cells from row i towards row W-1
-        for (int j = 0; j < L; j++) hist[j] = 0;
+        uint8_t hist_l[BIG ? 1 : 32];  // histogram row i: free cells from row i towards row W-1
+        extern __shared__ __align__(16) unsigned char heur_dyn[];
+        uint8_t *const hist_s = heur_dyn + heur_big_map_bytes(W, L) + threadIdx.x;
+        auto hist = [&](int j) -> uint8_t & { return BIG ? hist_s[j * FEAS_THREADS] : hist_l[j]; };
+        for (int j = 0; j < L; j++) hist(j) = 0;
         int best = 0;
         for (int i = W - 1; i >= 0; i--) {
             for (int j = 0; j < L; j++) {
                 const bool in = i >= k.lx && i < k.lx + k.sx && j >= k.ly && j < k.ly + k.sy;
                 const bool fr = (in ? top : (int)hm[i * L + j]) <= lev;
-                hist[j] = fr ? (uint8_t)(hist[j] + 1) : (uint8_t)0;
+                hist(j) = fr ? (uint8_t)(hist(j) + 1) : (uint8_t)0;
             }
             for (int j = 0; j < L; j++) {
-                const int v = hist[j];
-                if (v == 0 || (j > 0 && v == hist[j - 1])) continue;
+                const int v = hist(j);
+                if (v == 0 || (j > 0 && v == hist(j - 1))) continue;
                 int j2 = j, j1 = j;
-                while (j2 != L - 1 && !(hist[j2 + 1] < v)) j2++;
-                while (j1 != 0 && !(hist[j1 - 1] < v)) j1--;
+                while (j2 != L - 1 && !(hist(j2 + 1) < v)) j2++;
+                while (j1 != 0 && !(hist(j1 - 1) < v)) j1--;
                 best = max(best, v * (j2 - j1 + 1));
             }
         }
@@ -111,15 +126,19 @@ __device__ __noinline__ long long macs_score(const int16_t *hm, int W, int L, co
     return score;
 }
 
-template <bool STAB>
+// BIG (see heur_big_smem): launched with the dynamic shared memory of the container, for HM / MACS / RANDOM only.
+template <bool STAB, bool BIG>
 __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DParams p, const HParams hp) {
     __shared__ __align__(16) unsigned char sm[K3_SMEM];
-    __shared__ int16_t hm[HM_CELLS_MAX];
+    __shared__ int16_t hm_s[BIG ? 1 : HM_CELLS_MAX];
     __shared__ uint8_t ord[E_MAX];
     __shared__ int c_feas[FEAS_THREADS], c_mh[FEAS_THREADS];
     __shared__ long long c_score[FEAS_THREADS];
-    __shared__ uint32_t fbits[HC_MAX / 32];
+    __shared__ uint32_t fbits_s[BIG ? 1 : HC_MAX / 32];
     __shared__ int hm_sum, stop;
+    extern __shared__ __align__(16) unsigned char heur_dyn[];
+    int16_t *const hm = BIG ? (int16_t *)heur_dyn : hm_s;
+    uint32_t *const fbits = BIG ? (uint32_t *)(heur_dyn + heur_big_map_bytes(p.W, p.L)) : fbits_s;
     const int tid = threadIdx.x, lane = tid & 31;
     const int code = hp.code;
     const int e = code == PCT_H_QUERY_ ? hp.q_env : blockIdx.x;
@@ -225,8 +244,8 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
         if (ny < 1) ny = 1;
     }
     if (code == PCT_H_RANDOM) {
-        if (n_c > HC_MAX) n_c = HC_MAX;
-        for (int w = tid; w < HC_MAX / 32; w += FEAS_THREADS) fbits[w] = 0;
+        if (!BIG && n_c > HC_MAX) n_c = HC_MAX;  // BIG: the bitmap holds every grid candidate
+        for (int w = tid; w < (BIG ? (n_c + 31) / 32 : HC_MAX / 32); w += FEAS_THREADS) fbits[w] = 0;
         __syncthreads();
     }
     // LSAH footprint state; a fresh episode (no box placed yet) starts from the empty footprint
@@ -272,7 +291,7 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
                     }
                     score = (long long)k.ex * k.ey * k.ez + fits + (fits == p.n_items ? 10 : 0);
                 } else if (code == PCT_H_MACS) {
-                    score = macs_score(hm, W, L, k, mh);
+                    score = macs_score<BIG>(hm, W, L, k, mh);
                 } else if (code == PCT_H_DBL) {  // heuristic.py:482
                     score = k.lx + k.ly + 100ll * mh;
                 } else if (code == PCT_H_HM) {  // heuristic.py:281: 100 * np.sum(height map after the placement)
@@ -347,9 +366,22 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
 
 cudaError_t launch_heuristic_discrete(const DParams &p, const HParams &hp, cudaStream_t st) {
     const int grid = hp.code == PCT_H_QUERY_ ? 1 : p.n_envs;
-    if (p.setting == 2) pct_heuristic_kernel<false><<<grid, FEAS_THREADS, 0, st>>>(p, hp);
-    else pct_heuristic_kernel<true><<<grid, FEAS_THREADS, 0, st>>>(p, hp);
+    if ((p.W > HEUR_SIDE_MAX || p.L > HEUR_SIDE_MAX) && (hp.code == PCT_H_HM || hp.code == PCT_H_MACS || hp.code == PCT_H_RANDOM)) {
+        const size_t smem = heur_big_smem(p.W, p.L, p.setting == 2 ? 6 : 2);
+        if (p.setting == 2) pct_heuristic_kernel<false, true><<<grid, FEAS_THREADS, smem, st>>>(p, hp);
+        else pct_heuristic_kernel<true, true><<<grid, FEAS_THREADS, smem, st>>>(p, hp);
+    } else if (p.setting == 2) pct_heuristic_kernel<false, false><<<grid, FEAS_THREADS, 0, st>>>(p, hp);
+    else pct_heuristic_kernel<true, false><<<grid, FEAS_THREADS, 0, st>>>(p, hp);
     return cudaGetLastError();
+}
+
+// the dynamic shared memory limit of the large-container instantiations, raised to what the largest container needs (pct_create of a
+// discrete handle with W or L > 32; idempotent), so that launch_heuristic_discrete only enqueues
+cudaError_t prepare_heuristic_big() {
+    const int smem = (int)heur_big_smem(255, 255, 6);
+    cudaError_t e = cudaFuncSetAttribute(pct_heuristic_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(pct_heuristic_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    return e;
 }
 
 }  // namespace pct

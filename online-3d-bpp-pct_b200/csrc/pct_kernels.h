@@ -252,8 +252,9 @@ struct HParamsC {
     double *q_out;
 };
 constexpr int PCT_H_QUERY_ = 7;
-constexpr int HEUR_SIDE_MAX = 32;  // height-map based codes (HM, MACS, RANDOM's bitmap, single discrete query): W, L <= 32
+constexpr int HEUR_SIDE_MAX = 32;  // static height map of the heuristic kernel (single discrete query: W, L <= 32; HM / MACS / RANDOM above it: BIG instantiation)
 cudaError_t launch_heuristic_discrete(const DParams &p, const HParams &hp, cudaStream_t st);
+cudaError_t prepare_heuristic_big();  // pct_create of a discrete handle with W or L > HEUR_SIDE_MAX
 
 // batched placement queries (pct_query.cuh; continuous: pct_heuristics_continuous.cuh): row r asks k placements of env env[r]
 struct QParams {

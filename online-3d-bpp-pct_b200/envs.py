@@ -38,15 +38,36 @@ class _SpaceView(object):
     def plain_size(self):
         return np.array(self._env.bin_size)
 
+    def _wide(self):
+        """a discrete bin with a side above 32 cells: the single query (pct_query_placement) refuses it, the batched calls do not"""
+        return not self._env._continuous and max(int(self._env.bin_size[0]), int(self._env.bin_size[1])) > 32
+
     @property
     def plain(self):  # the height map (D:space.py:316-326)
         W, L = int(self._env.bin_size[0]), int(self._env.bin_size[1])
+        if self._wide():
+            return self._env._batch.height_maps([0])[0].cpu().numpy()
         return self._env._batch.query_placement(0, (1, 1, 0), 0, 0, want_map=True)[2][:W, :L]
+
+    def _query_wide(self, x, y, z, lx, ly, density, want_map):
+        """the single query's answer from the batched calls: one placement of env 0, and the map with the footprint (the part inside
+        the bin) raised to rest height + z, which is Space.update_height_graph on a copy (D:space.py:316-326)"""
+        b = self._env._batch
+        feas, rest = b.query_placements(torch.tensor([[[x, y, z, lx, ly]]]), env_idx=[0], density=[[float(density)]])
+        feas, rest = bool(feas.item()), int(rest.item())
+        if not want_map:
+            return feas, rest
+        hm = b.height_maps([0])[0].cpu().numpy()
+        hm[max(lx, 0):max(lx + x, 0), max(ly, 0):max(ly + y, 0)] = rest + z
+        return feas, rest, hm
 
     def drop_box_virtual(self, box_size, idx, flag, density, setting, returnH=False, returnMap=False):
         """D:space.py:393-433 — what heuristic.py asks for every placement it considers"""
         x, y, z = box_size if not flag else (box_size[1], box_size[0], box_size[2])
-        res = self._env._batch.query_placement(0, (x, y, z), idx[0], idx[1], density=density, want_map=returnMap and not returnH)
+        if self._wide():
+            res = self._query_wide(int(x), int(y), int(z), int(idx[0]), int(idx[1]), density, returnMap and not returnH)
+        else:
+            res = self._env._batch.query_placement(0, (x, y, z), idx[0], idx[1], density=density, want_map=returnMap and not returnH)
         if returnH:
             return res[0], res[1]
         if returnMap:
