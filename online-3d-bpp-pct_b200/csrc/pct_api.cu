@@ -43,6 +43,35 @@ cudaError_t launch_snapshot(pct_env_batch *h, const int32_t *env, int n, void *b
 cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, void *obs, cudaStream_t st);
 }  // namespace pct
 
+namespace pct {
+// the step's pools of stability walks: worst-case capacity, only the used prefix is ever touched.  Continuation pool: WalkCont entries for the
+// sequential kernel, the (larger) piece queue + its flags and per-walk counters only with PCT_B200_WALK=fork
+cudaError_t create_walk_pools(pct_env_batch *h, size_t item_bytes) {
+    const size_t n = (size_t)h->n_envs;
+    h->contq_env_bytes = h->walk_fork ? sizeof(WalkPiece) * (size_t)WALK_PIECES_PER_ENV : sizeof(WalkCont) * (size_t)WALK_CONT_PER_ENV;
+    cudaError_t e = cudaMalloc(&h->d_walkq, item_bytes * (size_t)CAND_MAX * n);
+    if (e == cudaSuccess) e = cudaMalloc(&h->d_walk_ctr, sizeof(int32_t) * n);
+    if (e == cudaSuccess) e = cudaMemset(h->d_walk_ctr, 0, sizeof(int32_t) * n);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&h->d_contq, h->contq_env_bytes * n);
+    if (e == cudaSuccess) e = cudaMalloc(&h->d_cont_ctr, sizeof(int32_t) * 8 * (n + 1));
+    if (e == cudaSuccess) e = cudaMemset(h->d_cont_ctr, 0, sizeof(int32_t) * 8 * (n + 1));
+    if (e == cudaSuccess && h->walk_fork) e = cudaMalloc(&h->d_piece_ready, sizeof(int32_t) * (size_t)WALK_PIECES_PER_ENV * n);
+    if (e == cudaSuccess && h->walk_fork) e = cudaMemset(h->d_piece_ready, 0, sizeof(int32_t) * (size_t)WALK_PIECES_PER_ENV * n);
+    if (e == cudaSuccess && h->walk_fork) e = cudaMalloc(&h->d_walk_pend, sizeof(int32_t) * (size_t)CAND_MAX * n);
+    return e;
+}
+
+cudaError_t sm_count(int *n) {
+    static int n_sm = 0;
+    int dev = 0;
+    cudaError_t e = cudaSuccess;
+    if (!n_sm) e = cudaGetDevice(&dev);
+    if (!n_sm && e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    *n = n_sm;
+    return e;
+}
+}  // namespace pct
+
 extern "C" {
 
 const char *pct_version(void) { return "pct_b200 0.1 (sm_90a)"; }
@@ -148,19 +177,7 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
             // HM / MACS / RANDOM on a bin wider than 32 cells run with dynamic shared memory: raise its limit here, so that
             // pct_heuristic_actions stays enqueue-only (capturable)
             if (e == cudaSuccess && (cfg->container_size[0] > HEUR_SIDE_MAX || cfg->container_size[1] > HEUR_SIDE_MAX)) e = prepare_heuristic_big();
-            if (e == cudaSuccess && !h->k3_block) {  // the step's pool of stability walks: worst-case capacity, only the used prefix is ever touched
-                e = cudaMalloc(&h->d_walkq, sizeof(WalkItem) * (size_t)CAND_MAX * (size_t)n_envs);
-                if (e == cudaSuccess) e = cudaMalloc(&h->d_walk_ctr, sizeof(int32_t) * (size_t)n_envs);
-                if (e == cudaSuccess) e = cudaMemset(h->d_walk_ctr, 0, sizeof(int32_t) * (size_t)n_envs);
-                // continuation pool: WalkCont entries for the sequential kernel, the (larger) piece queue + its flags and per-walk counters only with PCT_B200_WALK=fork
-                h->contq_env_bytes = h->walk_fork ? sizeof(WalkPiece) * (size_t)WALK_PIECES_PER_ENV : sizeof(WalkCont) * (size_t)WALK_CONT_PER_ENV;
-                if (e == cudaSuccess) e = cudaMalloc((void **)&h->d_contq, h->contq_env_bytes * (size_t)n_envs);
-                if (e == cudaSuccess) e = cudaMalloc(&h->d_cont_ctr, sizeof(int32_t) * 8 * ((size_t)n_envs + 1));  // eight counters per (possible) env range
-                if (e == cudaSuccess) e = cudaMemset(h->d_cont_ctr, 0, sizeof(int32_t) * 8 * ((size_t)n_envs + 1));
-                if (e == cudaSuccess && h->walk_fork) e = cudaMalloc(&h->d_piece_ready, sizeof(int32_t) * (size_t)WALK_PIECES_PER_ENV * (size_t)n_envs);
-                if (e == cudaSuccess && h->walk_fork) e = cudaMemset(h->d_piece_ready, 0, sizeof(int32_t) * (size_t)WALK_PIECES_PER_ENV * (size_t)n_envs);
-                if (e == cudaSuccess && h->walk_fork) e = cudaMalloc(&h->d_walk_pend, sizeof(int32_t) * (size_t)CAND_MAX * (size_t)n_envs);
-            }
+            if (e == cudaSuccess && !h->k3_block) e = create_walk_pools(h, sizeof(WalkItem));
             h->lpt = !h->k3_block;   // heaviest-env-first block order (pct_discrete.cu, order_lookup / order_file); PCT_B200_LPT=0 disables
             if (const char *lv = getenv("PCT_B200_LPT")) h->lpt = atoi(lv) != 0 && !h->k3_block;
             if (e == cudaSuccess && h->lpt) {
@@ -293,14 +310,7 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
         prof = &h->prof_ev[(size_t)h->prof_steps * 4];
         h->prof_steps++;
     }
-    p.walkq = h->d_walkq ? h->d_walkq + (size_t)off * CAND_MAX : nullptr;  // env ranges stepped concurrently (pct_step_host's staged path) own disjoint slices
-    p.walk_ctr = h->d_walk_ctr ? h->d_walk_ctr + off : nullptr;
-    p.contq = h->d_contq ? (WalkCont *)((char *)h->d_contq + (size_t)off * h->contq_env_bytes) : nullptr;  // an env range's slice of the pool
-    p.cont_ctr = h->d_cont_ctr ? h->d_cont_ctr + 8 * (size_t)off : nullptr;
-    p.walk_lanes = h->walk_lanes; p.walk_lanes_tall = h->walk_lanes_tall;
-    p.walk_fork = h->walk_fork ? 1 : 0; p.walk_blocks = h->walk_blocks; p.walk_keep = h->walk_keep; p.piece_cap = cnt * WALK_PIECES_PER_ENV;
-    p.piece_ready = h->d_piece_ready ? h->d_piece_ready + (size_t)off * WALK_PIECES_PER_ENV : nullptr;
-    p.walk_pend = h->d_walk_pend ? h->d_walk_pend + (size_t)off * CAND_MAX : nullptr;
+    p.walk = walk_pools<WalkItem>(h, off, cnt);
     if (pre) CK(h, pre->items ? launch_set_items_discrete(p, *pre->items, gs) : launch_reset_envs_discrete(p, *pre->reset, gs));
     else CK(h, launch_discrete(p, gs, prof));
     h->launches += discrete_kernels_per_step(p);

@@ -15,7 +15,7 @@
 #include "pct_kernels.h"
 #include "pct_handle.h"
 #include "pct_geom_continuous.cuh"
-#include "pct_walkq.cuh"
+#include "pct_walks.cuh"
 #include "pct_continuous.cuh"
 
 namespace pct {
@@ -559,7 +559,7 @@ __global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
         shuffle_candidates<uint16_t>(ev->cand, cnt, (uint64_t *)ev->ems_tmp, (uint16_t *)((char *)ev->ems_tmp + 10240), p.seed, (uint64_t)(p.env_id_base + e),
                                      (uint64_t)h.draw_pos, lane);
     }
-    if (p.walkq) {
+    if (p.walk.walkq) {
         // ---- classify (round 2): drop_box_virtual's bounds / resting height (C:space.py:380-398) on pre-rounded box rectangles, supports + exact
         // quick reject for the placements that rest on boxes; the stability walks of all envs go to one pool (pctc_walk_light / pctc_walk kernels) ----
         __shared__ double rb[NB_MAX][5];
@@ -619,9 +619,9 @@ __global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
             n_walk += __popc(pm);
             if (pm) {
                 int qb = 0;
-                if (lane == 0) qb = atomicAdd(p.walk_ctr, __popc(pm));
+                if (lane == 0) qb = atomicAdd(p.walk.walk_ctr, __popc(pm));
                 qb = __shfl_sync(FULL, qb, 0);
-                if (pend) p.walkq[qb + __popc(pm & lt)] = WalkItemC{(uint32_t)e, pack, (uint16_t)c, code, k, mh};
+                if (pend) p.walk.walkq[qb + __popc(pm & lt)] = WalkItemC{(uint32_t)e, pack, (uint16_t)c, code, k, mh};
             }
             pos += 32;
         }
@@ -634,182 +634,44 @@ __global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
     }
 }
 
-// ---- pooled walks (round 2): see pct_discrete.cu — light prefix for every walk, continuation kernel for the walks that reach a node with >= 2 supports ----
-struct WalkViewC {
+// ---- pooled walks (round 2): the walk stage of pct_walks.cuh over the continuous record ----
+// the candidate's tuple is rebuilt from its code (cand_tuple); everything else of the walk lives in CEnv
+struct CWalkView {
     GeomC g;
     EdgePool pool;
     NodeC root;
     CEnv *ev;
+    __device__ __forceinline__ uint32_t *fbits() const { return ev->fbits; }
+    __device__ __forceinline__ int32_t *flags() const { return &ev->h.flags; }
+    __device__ __forceinline__ int32_t *n_pending() const { return &ev->n_pending; }
+    __device__ __forceinline__ BigScratch *big() const { return &ev->big; }
+    __device__ __forceinline__ int32_t *lock() const { return &ev->lock; }
 };
-__device__ __forceinline__ WalkViewC walk_view_c(const CParams &p, const WalkItemC &it, bool has) {
-    CEnv *ev = p.env + it.env;
-    const CHdr &h = ev->h;
-    double t6[6] = {0, 0, 0, 0, 0, 0};
-    if (has) {
-        const double nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
-        cand_tuple(it.code, ev->ems, nb, t6);
-    }
-    const double x = t6[3] - t6[0], y = t6[4] - t6[1], z = t6[5] - t6[2];
-    return WalkViewC{GeomC{ev->box, ev->den, has ? h.n_box : 0},
-                     EdgePool{ev->e_lower, ev->e_next, ev->e_off, ev->first_in, ev->last_in, ev->e_st, ev->e_st, has ? h.n_edge : 0, ev->poly_off,
-                              &ev->poly[0][0], &ev->poly[0][0], has ? h.n_poly : 0},
-                     NodeC{t6[0], t6[1], it.mh, x, y, z, x * y * z * (has ? h.next_den : 1.0)}, ev};
-}
-
-__global__ void __launch_bounds__(128, 4) pctc_walk_light_kernel(const CParams p) {
-    const int lane = threadIdx.x & 31;
-    const int total = *(volatile const int32_t *)p.walk_ctr;
-    const int nwarps = gridDim.x * 4;
-    const int cap = p.n_envs * WALK_CONT_PER_ENV;
-#pragma unroll 1
-    for (int base = (blockIdx.x * 4 + (threadIdx.x >> 5)) * 32; base < total; base += nwarps * 32) {
-        const int i = base + lane;
-        const bool has = i < total;
-        WalkItemC it{};
-        if (has) it = p.walkq[i];
-        const WalkViewC v = walk_view_c(p, it, has);
-        int node = NODE_NEW, res = 0;
-        Stack4 st{};
-        if (has) res = stab_light<GeomC>(v.g, v.root, it.k, it.pack, v.pool, node, st);
-        if (res == 1) atomicOr(&v.ev->fbits[it.c >> 5], 1u << (it.c & 31));
-        if (has && res != 2) { __threadfence(); atomicSub(&v.ev->n_pending, 1); }
-        if (p.walk_fork) {  // fork-join continuation kernel: one queue of pieces (pct_walkq.cuh)
-            const uint32_t pm = __ballot_sync(FULL, res == 2);
-            if (pm) {
-                const PieceQueue pq{(WalkPiece *)p.contq, p.piece_ready, p.cont_ctr, p.piece_cap};
-                int qb = 0;
-                if (lane == 0) qb = pq_reserve_initial(pq, __popc(pm));
-                qb = __shfl_sync(FULL, qb, 0);
-                if (res == 2) {
-                    const int idx = qb + __popc(pm & ((1u << lane) - 1));
-                    if (idx < pq.cap) {
-                        p.walk_pend[i] = 1;
-                        pq.q[idx] = WalkPiece{(uint32_t)i, (uint8_t)node, (uint8_t)EDGE_NIL, 0, 0, st.cx, st.cy, st.m};
-                    } else {
-                        atomicOr(&v.ev->h.flags, PCT_FLAG_CAND_OVERFLOW);
-                        __threadfence();
-                        atomicSub(&v.ev->n_pending, 1);
-                        pq_piece_done(pq);
-                    }
-                }
-            }
-            continue;
+struct CWalk {
+    typedef CParams Params;
+    typedef WalkItemC Item;
+    typedef GeomC Geom;
+    static __device__ __forceinline__ CWalkView view(const CParams &p, const WalkItemC &it, bool has) {
+        CEnv *ev = p.env + it.env;
+        const CHdr &h = ev->h;
+        double t6[6] = {0, 0, 0, 0, 0, 0};
+        if (has) {
+            const double nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
+            cand_tuple(it.code, ev->ems, nb, t6);
         }
-        const bool tall = it.mh >= 0.6 * p.H;  // the longest chains: pooled from the end, fewer lanes per warp (see pct_discrete.cu)
-        const uint32_t ps = __ballot_sync(FULL, res == 2 && !tall), pt = __ballot_sync(FULL, res == 2 && tall);
-        if (ps | pt) {
-            int qs = 0, qt = 0;
-            if (lane == 0) {
-                if (ps) qs = atomicAdd(p.cont_ctr, __popc(ps));
-                if (pt) qt = atomicAdd(p.cont_ctr + 1, __popc(pt));
-            }
-            qs = __shfl_sync(FULL, qs, 0);
-            qt = __shfl_sync(FULL, qt, 0);
-            if (res == 2) {
-                const uint32_t lt = (1u << lane) - 1;
-                const int idx = tall ? qt + __popc(pt & lt) : qs + __popc(ps & lt);
-                if (idx < cap / 2) p.contq[tall ? cap - 1 - idx : idx] = WalkCont{(uint32_t)i, (uint32_t)node, st};
-                else { atomicOr(&v.ev->h.flags, PCT_FLAG_CAND_OVERFLOW); __threadfence(); atomicSub(&v.ev->n_pending, 1); }
-            }
-        }
+        const double x = t6[3] - t6[0], y = t6[4] - t6[1], z = t6[5] - t6[2];
+        return CWalkView{GeomC{ev->box, ev->den, has ? h.n_box : 0},
+                               EdgePool{ev->e_lower, ev->e_next, ev->e_off, ev->first_in, ev->last_in, ev->e_st, ev->e_st, has ? h.n_edge : 0, ev->poly_off,
+                                        &ev->poly[0][0], &ev->poly[0][0], has ? h.n_poly : 0},
+                               NodeC{t6[0], t6[1], it.mh, x, y, z, x * y * z * (has ? h.next_den : 1.0)},
+                         ev};
     }
-}
-
-__global__ void __launch_bounds__(64, 8) pctc_walk_kernel(const CParams p) {
-    const int lane = threadIdx.x & 31;
-    const int cap = p.n_envs * WALK_CONT_PER_ENV;
-    const int n_short = min(*(volatile const int32_t *)p.cont_ctr, cap / 2), n_tall = min(*(volatile const int32_t *)(p.cont_ctr + 1), cap / 2);
-    __syncthreads();
-    pdl_launch_dependents();  // the emit kernel may follow: its blocks wait for their env's last walk (CEnv::n_pending)
-    const int nwarps = gridDim.x * 2, Ls = p.walk_lanes, Lt = p.walk_lanes_tall;
-    const int w_tall = (n_tall + Lt - 1) / Lt, w_all = w_tall + (n_short + Ls - 1) / Ls;
-#pragma unroll 1
-    for (int w = blockIdx.x * 2 + (threadIdx.x >> 5); w < w_all; w += nwarps) {
-        const bool tw = w < w_tall;
-        const int L = tw ? Lt : Ls;
-        const unsigned mask = L >= 32 ? FULL : ((1u << L) - 1u);
-        if (lane >= L) continue;
-        const int i = tw ? w * Lt + lane : (w - w_tall) * Ls + lane;
-        const bool has = i < (tw ? n_tall : n_short);
-        WalkCont ct{};
-        WalkItemC it{};
-        if (has) { ct = p.contq[tw ? cap - 1 - i : i]; it = p.walkq[ct.item]; }
-        const WalkViewC v = walk_view_c(p, it, has);
-        int fl = 0;
-        const bool ok = stab_virtual<GeomC>(v.g, v.root, it.k, it.pack, v.pool, &v.ev->big, &v.ev->lock, fl, has, mask, has ? (int)ct.node : NODE_NEW, &ct.st) != 0;
-        if (has && ok) atomicOr(&v.ev->fbits[it.c >> 5], 1u << (it.c & 31));
-        if (has && fl) atomicOr(&v.ev->h.flags, fl);
-        if (has) { __threadfence(); atomicSub(&v.ev->n_pending, 1); }
-    }
-}
-
-// fork-join form of the continuation kernel: see pct_walk_fork_kernel (pct_discrete.cu) and pct_walkq.cuh — same protocol, continuous geometry
-struct PieceForkC {
-    PieceQueue pq;
-    int32_t *pend;
-    uint32_t item;
-    int n_init;
-    bool overflow;
-    __device__ __forceinline__ void operator()(int child, int skip, double vx, double vy, double vm) {
-        if (!pq_fork(pq, n_init, pend, WalkPiece{item, (uint8_t)child, (uint8_t)skip, 1, 0, vx, vy, vm})) overflow = true;
-    }
+    static __device__ __forceinline__ bool tall(const CParams &p, const WalkItemC &it) { return it.mh >= 0.6 * p.H; }
 };
-__device__ __forceinline__ void run_piece_c(const CParams &p, const PieceQueue &pq, int n_init, int slot) {
-    const WalkPiece pc = pq.q[slot];
-    if (slot >= n_init) pq.ready[slot] = 0;
-    const WalkItemC it = p.walkq[pc.item];
-    const WalkViewC v = walk_view_c(p, it, true);
-    int32_t *pend = p.walk_pend + pc.item;
-    int fl = 0, ok = 0;
-    if (!(*(volatile const int32_t *)pend & WALK_FAILED)) {
-        PieceForkC fork{pq, pend, pc.item, n_init, false};
-        ok = stab_piece<GeomC>(v.g, v.root, it.k, it.pack, v.pool, &v.ev->big, &v.ev->lock, fl, (int)pc.node, (int)pc.kind, (int)pc.skip, pc.a, pc.b, pc.c, fork);
-        if (fork.overflow) { fl |= PCT_FLAG_CAND_OVERFLOW; ok = 0; }
-    }
-    if (fl) atomicOr(&v.ev->h.flags, fl);
-    if (!ok) atomicOr(pend, WALK_FAILED);
-    __threadfence();
-    const int r = atomicSub(pend, 1);
-    if ((r & (WALK_FAILED - 1)) == 1) {
-        if (!(r & WALK_FAILED)) atomicOr(&v.ev->fbits[it.c >> 5], 1u << (it.c & 31));
-        __threadfence();
-        atomicSub(&v.ev->n_pending, 1);
-    }
-    pq_piece_done(pq);
-}
-__global__ void __launch_bounds__(64, 8) pctc_walk_fork_kernel(const CParams p) {
-    const int lane = threadIdx.x & 31;
-    const int wid = blockIdx.x * 2 + (threadIdx.x >> 5), n_warps = gridDim.x * 2;
-    const PieceQueue pq{(WalkPiece *)p.contq, p.piece_ready, p.cont_ctr, p.piece_cap};
-    const int n_init = min(*(volatile const int32_t *)(pq.ctr + PQ_NINIT), pq.cap);
-    const int L = p.walk_lanes;
-    pdl_launch_dependents();
-    if (n_init > 0) {
-#pragma unroll 1
-        for (int b = wid * L; b < n_init; b += n_warps * L) {
-            if (lane < L && b + lane < n_init) run_piece_c(p, pq, n_init, b + lane);
-            __syncwarp();
-        }
-        const bool keep = wid < p.walk_keep;
-#pragma unroll 1
-        for (;;) {
-            int t0 = -1;
-            if (lane == 0 && (keep || *(volatile const int32_t *)(pq.ctr + PQ_ALLOC) - *(volatile const int32_t *)(pq.ctr + PQ_HEAD) > 0))
-                t0 = atomicAdd(pq.ctr + PQ_HEAD, L);
-            t0 = __shfl_sync(FULL, t0, 0);
-            if (t0 < 0) break;
-            bool fin = false;
-            if (lane < L) {
-                const int slot = n_init + t0 + lane;
-                if (pq_wait(pq, slot)) run_piece_c(p, pq, n_init, slot);
-                else fin = true;
-            }
-            __syncwarp();
-            if (__any_sync(FULL, fin)) break;
-        }
-    }
-    if (lane == 0) pq_warp_exit(pq, n_warps, p.walk_ctr);
-}
+
+__global__ void __launch_bounds__(32 * LIGHT_WARPS, 4) pctc_walk_light_kernel(const CParams p) { walk_light<CWalk>(p); }
+__global__ void __launch_bounds__(32 * WALK_WARPS, 8) pctc_walk_kernel(const CParams p) { PCT_WALK_CONT_BODY(CWalk, p) }
+__global__ void __launch_bounds__(32 * WALK_WARPS, 8) pctc_walk_fork_kernel(const CParams p) { walk_fork<CWalk>(p); }
 
 template <typename OT> __device__ __noinline__ void write_obs_c_delta(const CParams &p, int e, const CEnv *ev, const double (*leaf)[6], int n_leaf, int tid, int nthreads);
 
@@ -822,15 +684,8 @@ __global__ void __launch_bounds__(64) pctc_emit_kernel(const CParams p) {
     CEnv *ev = p.env + e;
     const CHdr &h = ev->h;
     const double nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
-    if (e == 0 && tid == 0 && !p.walk_fork) { *p.walk_ctr = 0; p.cont_ctr[0] = 0; p.cont_ctr[1] = 0; }  // every walk-kernel block has read them (programmatic dependency): empty the pools for the next step
-    if (tid == 0) {  // may run while this env's walks are still in flight (programmatic dependent of the continuation kernel)
-        int spins = 0;
-        while (*(volatile const int32_t *)&ev->n_pending > 0) {
-            __nanosleep(spins < 16 ? 100 : 1000);
-            if (++spins > (1 << 22)) { atomicOr(&ev->h.flags, PCT_FLAG_SYNC_TIMEOUT); break; }
-        }
-        __threadfence();
-    }
+    if (e == 0 && tid == 0) reset_walk_pools(p.walk);
+    if (tid == 0) wait_walks(&ev->n_pending, ev);
     __syncthreads();
     if (tid < 32) {
         const int nl = p.nl, nw = ev->n_fw;
@@ -1068,20 +923,11 @@ int continuous_create(pct_env_batch *h) {
     if (e == cudaSuccess) e = cudaMemset(h->c_state, 0, sizeof(CEnv) * (size_t)h->n_envs);
     if (e == cudaSuccess) e = cudaMalloc(&h->d_ready, sizeof(int32_t) * 2 * (size_t)h->n_envs);
     if (e == cudaSuccess) e = cudaMemset(h->d_ready, 0, sizeof(int32_t) * 2 * (size_t)h->n_envs);
-    if (e == cudaSuccess && !h->k3_block) {  // pools of the round-2 walk kernels (worst-case capacity for the walks; only the used prefix is touched)
-        e = cudaMalloc(&h->c_walkq, sizeof(WalkItemC) * (size_t)CAND_MAX * (size_t)h->n_envs);
-        if (e == cudaSuccess) e = cudaMalloc(&h->d_walk_ctr, sizeof(int32_t) * 16);  // [0] walk pool, [1..] continuation pool counters (sequential kernel: ordinary / tall; fork-join: pct_walkq.cuh)
-        if (e == cudaSuccess) e = cudaMemset(h->d_walk_ctr, 0, sizeof(int32_t) * 16);
-        if (e == cudaSuccess && h->walk_fork) e = cudaMalloc(&h->d_piece_ready, sizeof(int32_t) * (size_t)WALK_PIECES_PER_ENV * (size_t)h->n_envs);
-        if (e == cudaSuccess && h->walk_fork) e = cudaMemset(h->d_piece_ready, 0, sizeof(int32_t) * (size_t)WALK_PIECES_PER_ENV * (size_t)h->n_envs);
-        if (e == cudaSuccess && h->walk_fork) e = cudaMalloc(&h->d_walk_pend, sizeof(int32_t) * (size_t)CAND_MAX * (size_t)h->n_envs);
-        h->contq_env_bytes = h->walk_fork ? sizeof(WalkPiece) * (size_t)WALK_PIECES_PER_ENV : sizeof(WalkCont) * (size_t)WALK_CONT_PER_ENV;
-        if (e == cudaSuccess) e = cudaMalloc((void **)&h->d_contq, h->contq_env_bytes * (size_t)h->n_envs);
-    }
+    if (e == cudaSuccess && !h->k3_block) e = create_walk_pools(h, sizeof(WalkItemC));
     if (e != cudaSuccess) { h->err = std::string("continuous_create: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
     return PCT_OK;
 }
-void continuous_destroy(pct_env_batch *h) { cudaFree(h->c_state); h->c_state = nullptr; cudaFree(h->c_walkq); h->c_walkq = nullptr; }
+void continuous_destroy(pct_env_batch *h) { cudaFree(h->c_state); h->c_state = nullptr; }
 int64_t continuous_state_bytes() { return (int64_t)sizeof(CEnv); }
 
 // CParams of the whole batch for the kernels that only read the item source (pct_preview_items)
@@ -1140,27 +986,24 @@ int continuous_launch(pct_env_batch *h, int mode, const void *actions, int actio
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t cfg{};
     cfg.stream = st; cfg.attrs = at; cfg.numAttrs = p.ready ? 1 : 0;
-    const bool pooled = h->c_walkq != nullptr && !h->k3_block;
+    const bool pooled = h->d_walkq != nullptr;
     if (pooled && h->obs_delta && h->d_aux) {  // delta observation rows (emit kernel): a buffer other than the tracked one may hold anything -> "all rows"
         if (h->fill_pending) launch_fill_prev(h->d_aux, p.n_envs, p.nb, p.nl, st);
         p.aux = h->d_aux;
         p.delta = 1;
     }
     h->fill_pending = false;
-    if (pooled) {
-        p.walkq = (WalkItemC *)h->c_walkq; p.walk_ctr = h->d_walk_ctr; p.contq = h->d_contq; p.cont_ctr = h->d_walk_ctr + 1; p.walk_lanes = h->walk_lanes; p.walk_lanes_tall = h->walk_lanes_tall;
-        p.walk_fork = h->walk_fork ? 1 : 0; p.walk_blocks = h->walk_blocks; p.walk_keep = h->walk_keep; p.piece_cap = p.n_envs * WALK_PIECES_PER_ENV;
-        p.piece_ready = h->d_piece_ready; p.walk_pend = h->d_walk_pend;
-    }
+    if (pooled) p.walk = walk_pools<WalkItemC>(h, 0, p.n_envs);
     cfg.gridDim = dim3(p.n_envs); cfg.blockDim = dim3(32);
     cudaLaunchKernelEx(&cfg, pctc_candidates_kernel, p);
     if (pooled) {
-        static int n_sm = 0;
-        if (!n_sm) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); }
         if (stab) {
-            pctc_walk_light_kernel<<<n_sm * 4, 128, 0, st>>>(p);
-            if (p.walk_fork) pctc_walk_fork_kernel<<<n_sm * max(1, min(p.walk_blocks, 8)), 64, 0, st>>>(p);  // one resident wave
-            else pctc_walk_kernel<<<n_sm * 8, 64, 0, st>>>(p);  // one resident wave
+            int n_sm = 0;
+            const cudaError_t es = sm_count(&n_sm);
+            if (es != cudaSuccess) { h->err = std::string("continuous launch: ") + cudaGetErrorString(es); return PCT_ERR_CUDA; }
+            pctc_walk_light_kernel<<<n_sm * 4, 32 * LIGHT_WARPS, 0, st>>>(p);
+            if (p.walk.walk_fork) pctc_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, 8)), 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
+            else pctc_walk_kernel<<<n_sm * 8, 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
         }
         {
             cudaLaunchAttribute at2[1];

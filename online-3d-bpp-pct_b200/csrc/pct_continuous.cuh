@@ -69,16 +69,12 @@ struct CParams {
     int32_t *ready;  // overlapped launch mode: per-env hand-over flags [2 * n_envs] (see pct_common.cuh), nullptr = off
     int32_t epoch;
     int shuffle;     // pct_config::shuffle: keyed permutation of the ordered candidate list (shuffle_candidates)
-    WalkItemC *walkq;   // pooled stability walks (round 2, see pct_discrete.cu "K3 (round 2)"); nullptr: round 1's block kernel does everything
-    int32_t *walk_ctr;
-    WalkCont *contq;
-    int32_t *cont_ctr;
-    int32_t walk_lanes, walk_lanes_tall;
-    int32_t walk_fork, walk_blocks, walk_keep, piece_cap;   // fork-join continuation kernel (see DParams)
-    int32_t *piece_ready, *walk_pend;
+    WalkPools<WalkItemC> walk;  // pooled stability walks (round 2, pct_walks.cuh); walk.walkq nullptr: round 1's block kernel does everything
     int32_t delta;   // delta observation rows (DEnvAux::obs_prev), emit kernel only
     DEnvAux *aux;    // per-env state of the ALIAS apply kernel (EdgePoolA arrays), nullptr with PCT_B200_ALIAS=0 / setting 2
 };
+static_assert(sizeof(WalkPools<WalkItemC>) == 72 && offsetof(CParams, walk) == 232 && offsetof(CParams, delta) == 304 && sizeof(CParams) == 320,
+              "walk pools at the byte offsets of the fields they replaced");
 
 template <typename OT>
 __device__ __noinline__ void write_obs_c(const CParams &p, int e, const CEnv *ev, const double (*leaf)[6], int n_leaf, int tid, int nthreads) {

@@ -26,7 +26,7 @@
 #include "pct_stability.cuh"
 #include "pct_kernels.h"
 #include "pct_geom.cuh"
-#include "pct_walkq.cuh"
+#include "pct_walks.cuh"
 #include "pct_obs.cuh"
 
 namespace pct {
@@ -953,7 +953,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) pct_candidates_kernel(co
                                   (uint64_t)h.draw_pos, lane);
         cand = out;
     }
-    if (p.walkq) {
+    if (p.walk.walkq) {
         // ---- classify (round 2; see "K3 (round 2)" below): drop_box_virtual (D:space.py:393-433) + check_box (:436-454), integer part ----
         constexpr bool STAB = !BIGSM;
         const int n_box = h.n_box, nl = p.nl;
@@ -982,14 +982,14 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) pct_candidates_kernel(co
             n_walk += __popc(pm);
             if (pm) {
                 int qb = 0;
-                if (lane == 0) qb = atomicAdd(p.walk_ctr, __popc(pm));
+                if (lane == 0) qb = atomicAdd(p.walk.walk_ctr, __popc(pm));
                 qb = __shfl_sync(FULL, qb, 0);
                 if (pend) {
                     WalkItem it;
                     it.env = (uint32_t)e; it.pack = pack; it.c = (uint16_t)c;
                     it.xs = (uint8_t)xs; it.ys = (uint8_t)ys; it.mh = (uint8_t)mh; it.sx = (uint8_t)sx; it.sy = (uint8_t)sy; it.sz = (uint8_t)sz;
                     it.k = (uint8_t)min(k, 255); it.pad_ = 0;
-                    p.walkq[qb + __popc(pm & lt)] = it;
+                    p.walk.walkq[qb + __popc(pm & lt)] = it;
                 }
             }
             pos += 32;
@@ -1168,206 +1168,41 @@ __global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(co
 #ifndef LIGHT_MINB
 #define LIGHT_MINB 6
 #endif
-constexpr int WALK_WARPS = 2, LIGHT_WARPS = 4;
-
-// a walk of this env has delivered its verdict (fbits / flags written before): release-decrement the env's counter of running walks
-__device__ __forceinline__ void walk_done(int32_t *n_pending) {
-    __threadfence();
-    atomicSub(n_pending, 1);
-}
-
-// per-lane view of one pooled walk: the env's record stays in global memory (L1 / L2) — the lanes of a warp belong to different envs
-struct WalkView {
+// the discrete domain's side of the walk stage (pct_walks.cuh): hot record for the geometry, cold record for the walk's verdict and scratch
+struct DWalkView {
     GeomD g;
     EdgePool pool;
     NodeD root;
     DEnvCold *cold;
     const DEnvHot *hot;
+    __device__ __forceinline__ uint32_t *fbits() const { return cold->fbits; }
+    __device__ __forceinline__ int32_t *flags() const { return const_cast<int32_t *>(&hot->h.flags); }
+    __device__ __forceinline__ int32_t *n_pending() const { return &cold->n_pending; }
+    __device__ __forceinline__ BigScratch *big() const { return &cold->big; }
+    __device__ __forceinline__ int32_t *lock() const { return &cold->lock; }
 };
-__device__ __forceinline__ WalkView walk_view(const DParams &p, const WalkItem &it, bool has) {
-    const DEnvHot *hot = p.hot + it.env;
-    DEnvCold *cold = p.cold + it.env;
-    const DHdr &h = hot->h;
-    const int sx = it.sx, sy = it.sy, sz = it.sz;
-    return WalkView{GeomD{hot->box, has ? h.n_box : 0, p.setting == 3 ? cold->density : nullptr},
-                    EdgePool{const_cast<uint8_t *>(hot->e_lower), const_cast<uint8_t *>(hot->e_next), const_cast<uint16_t *>(hot->e_off),
-                             const_cast<uint8_t *>(hot->first_in), const_cast<uint8_t *>(hot->last_in), cold->e_st, cold->e_st, has ? h.n_edge : 0,
-                             const_cast<uint16_t *>(hot->poly_off), &cold->poly[0][0], &cold->poly[0][0], has ? h.n_poly : 0},
-                    NodeD{(int)it.xs, (int)it.ys, (int)it.mh, sx, sy, sz, (double)(sx * sy * sz) * (has ? h.next_den : 1.0)}, cold, hot};
-}
-
-// walk, stage 1: the light prefix of EVERY pooled walk, one lane per walk (stab_light: single-support visits only — small code, no local arrays).
-// 81 % of the walks end here; the rest goes to the continuation pool with (node, stack).
-__global__ void __launch_bounds__(32 * LIGHT_WARPS, LIGHT_MINB) pct_walk_light_kernel(const DParams p) {
-    const int lane = threadIdx.x & 31;
-    const int total = *(volatile const int32_t *)p.walk_ctr;
-    const int nwarps = gridDim.x * LIGHT_WARPS;
-    const int cap = p.n_envs * WALK_CONT_PER_ENV;
-#pragma unroll 1
-    for (int base = (blockIdx.x * LIGHT_WARPS + (threadIdx.x >> 5)) * 32; base < total; base += nwarps * 32) {
-        const int i = base + lane;
-        const bool has = i < total;
-        WalkItem it{};
-        if (has) it = p.walkq[i];
-        const WalkView v = walk_view(p, it, has);
-        int node = NODE_NEW, res = 0;
-        Stack4 st{};
-        if (has) res = stab_light<GeomD>(v.g, v.root, (int)it.k, it.pack, v.pool, node, st);
-        if (res == 1) atomicOr(&v.cold->fbits[it.c >> 5], 1u << (it.c & 31));
-        if (has && res != 2) walk_done(&v.cold->n_pending);
-        // continuations: walks high up in the bin descend through the deepest support DAGs (host statistics: resting height >= 0.6 H -> up to 8 heavy
-        // visits, below -> at most 2), so they are pooled apart (from the END of the pool) and get fewer lanes per warp in pct_walk_kernel
-        if (p.walk_fork) {  // fork-join continuation kernel: one queue of pieces, "enter `node` with the stack st" (pct_walkq.cuh)
-            const uint32_t pm = __ballot_sync(FULL, res == 2);
-            if (pm) {
-                const PieceQueue pq{(WalkPiece *)p.contq, p.piece_ready, p.cont_ctr, p.piece_cap};
-                int qb = 0;
-                if (lane == 0) qb = pq_reserve_initial(pq, __popc(pm));
-                qb = __shfl_sync(FULL, qb, 0);
-                if (res == 2) {
-                    const int idx = qb + __popc(pm & ((1u << lane) - 1));
-                    if (idx < pq.cap) {
-                        p.walk_pend[i] = 1;
-                        pq.q[idx] = WalkPiece{(uint32_t)i, (uint8_t)node, (uint8_t)EDGE_NIL, 0, 0, st.cx, st.cy, st.m};
-                    } else {  // never silent: the candidate stays infeasible and the env is flagged
-                        atomicOr(const_cast<int32_t *>(&v.hot->h.flags), PCT_FLAG_CAND_OVERFLOW);
-                        walk_done(&v.cold->n_pending);
-                        pq_piece_done(pq);
-                    }
-                }
-            }
-            continue;
-        }
-        const bool tall = (int)it.mh * 5 >= p.H * 3;
-        const uint32_t ps = __ballot_sync(FULL, res == 2 && !tall), pt = __ballot_sync(FULL, res == 2 && tall);
-        if (ps | pt) {
-            int qs = 0, qt = 0;
-            if (lane == 0) {
-                if (ps) qs = atomicAdd(p.cont_ctr, __popc(ps));
-                if (pt) qt = atomicAdd(p.cont_ctr + 1, __popc(pt));
-            }
-            qs = __shfl_sync(FULL, qs, 0);
-            qt = __shfl_sync(FULL, qt, 0);
-            if (res == 2) {
-                const uint32_t lt = (1u << lane) - 1;
-                const int idx = tall ? qt + __popc(pt & lt) : qs + __popc(ps & lt);  // each class owns half of the pool (the counters may overshoot; the consumer clamps)
-                if (idx < cap / 2) p.contq[tall ? cap - 1 - idx : idx] = WalkCont{(uint32_t)i, (uint32_t)node, st};
-                else { atomicOr(const_cast<int32_t *>(&v.hot->h.flags), PCT_FLAG_CAND_OVERFLOW); walk_done(&v.cold->n_pending); }  // never silent: the candidate stays infeasible and the env is flagged
-            }
-        }
+struct DWalk {
+    typedef DParams Params;
+    typedef WalkItem Item;
+    typedef GeomD Geom;
+    static __device__ __forceinline__ DWalkView view(const DParams &p, const WalkItem &it, bool has) {
+        const DEnvHot *hot = p.hot + it.env;
+        DEnvCold *cold = p.cold + it.env;
+        const DHdr &h = hot->h;
+        const int sx = it.sx, sy = it.sy, sz = it.sz;
+        return DWalkView{GeomD{hot->box, has ? h.n_box : 0, p.setting == 3 ? cold->density : nullptr},
+                               EdgePool{const_cast<uint8_t *>(hot->e_lower), const_cast<uint8_t *>(hot->e_next), const_cast<uint16_t *>(hot->e_off),
+                                        const_cast<uint8_t *>(hot->first_in), const_cast<uint8_t *>(hot->last_in), cold->e_st, cold->e_st, has ? h.n_edge : 0,
+                                        const_cast<uint16_t *>(hot->poly_off), &cold->poly[0][0], &cold->poly[0][0], has ? h.n_poly : 0},
+                               NodeD{(int)it.xs, (int)it.ys, (int)it.mh, sx, sy, sz, (double)(sx * sy * sz) * (has ? h.next_den : 1.0)},
+                         cold, hot};
     }
-}
-
-// walk, stage 2: the continuations — every lane starts with the heavy visit its walk stopped at, then runs the general light / heavy state
-// machine to the end of the walk.  Only `p.walk_lanes` lanes of a warp carry a walk (default 16; 4 for the walks resting at >= 0.6 H): there are few
-// continuations (3 per env) and each is a long serial chain; a full warp of them leaves
-// fewer warps than the SMs have schedulers, 4-8 per warp multiply the warp instructions (measured sweep).
-__global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_kernel(const DParams p) {
-    const int lane = threadIdx.x & 31;
-    const int cap = p.n_envs * WALK_CONT_PER_ENV;
-    const int n_short = min(*(volatile const int32_t *)p.cont_ctr, cap / 2), n_tall = min(*(volatile const int32_t *)(p.cont_ctr + 1), cap / 2);
-    __syncthreads();
-    pdl_launch_dependents();  // the emit kernel's blocks may become resident now (it also empties the pool counters: read above); each waits for ITS env's last walk
-    const int nwarps = gridDim.x * WALK_WARPS, Ls = p.walk_lanes, Lt = p.walk_lanes_tall;
-    const int w_tall = (n_tall + Lt - 1) / Lt, w_all = w_tall + (n_short + Ls - 1) / Ls;
-#pragma unroll 1
-    for (int w = blockIdx.x * WALK_WARPS + (threadIdx.x >> 5); w < w_all; w += nwarps) {  // the tall walks (longest chains) are dealt first
-        const bool tw = w < w_tall;
-        const int L = tw ? Lt : Ls;
-        const unsigned mask = L >= 32 ? FULL : ((1u << L) - 1u);
-        if (lane >= L) continue;
-        const int i = tw ? w * Lt + lane : (w - w_tall) * Ls + lane;
-        const bool has = i < (tw ? n_tall : n_short);
-        WalkCont ct{};
-        WalkItem it{};
-        if (has) { ct = p.contq[tw ? cap - 1 - i : i]; it = p.walkq[ct.item]; }
-        const WalkView v = walk_view(p, it, has);
-        int fl = 0;
-        const bool ok = stab_virtual<GeomD>(v.g, v.root, (int)it.k, it.pack, v.pool, &v.cold->big, &v.cold->lock, fl, has, mask,
-                                            has ? (int)ct.node : NODE_NEW, &ct.st) != 0;
-        if (has && ok) atomicOr(&v.cold->fbits[it.c >> 5], 1u << (it.c & 31));
-        if (has && fl) atomicOr(const_cast<int32_t *>(&v.hot->h.flags), fl);
-        if (has) walk_done(&v.cold->n_pending);
-    }
-}
-
-// walk, stage 2, fork-join form (opt-in, PCT_B200_WALK=fork): the queue holds PIECES of walks (stab_piece: one chain of visits; a node with k >= 2 supports keeps
-// its first subtree and publishes the other k - 1 as new pieces; protocol: pct_walkq.cuh).  A walk's verdict is the AND over its pieces:
-// walk_pend[item] counts them, the piece that brings it to zero sets the feasibility bit (unless one failed) and releases the env's n_pending.
-// The critical chain of a step's longest walk becomes its longest root-to-floor PATH instead of the sum over its visits (host statistics,
-// scratch/stats_paths.py: 51 -> 34 visit units at the 99.99 % quantile) — and the stage did not get faster in
-// measurements, whatever the number of helper warps, blocks per SM or pieces per warp: the continuation stage is bound by the issue rate of a few
-// hundred divergent, latency-bound warps (warp instructions = thread instructions / 4.8 lanes, ~10 cycles each), not by its longest walk.  Kept as an
-// opt-in because it is the measured answer to "would independent subtrees on separate lanes help?" and is parity-tested (tests/test_gpu_walk_fork.py).
-struct PieceFork {
-    PieceQueue pq;
-    int32_t *pend;
-    uint32_t item;
-    int n_init;
-    bool overflow;
-    __device__ __forceinline__ void operator()(int child, int skip, double vx, double vy, double vm) {
-        if (!pq_fork(pq, n_init, pend, WalkPiece{item, (uint8_t)child, (uint8_t)skip, 1, 0, vx, vy, vm})) overflow = true;
-    }
+    static __device__ __forceinline__ bool tall(const DParams &p, const WalkItem &it) { return (int)it.mh * 5 >= p.H * 3; }
 };
-// one piece: the chain of visits, then the walk's AND-reduction (walk_pend) and the queue's bookkeeping
-__device__ __forceinline__ void run_piece(const DParams &p, const PieceQueue &pq, int n_init, int slot) {
-    const WalkPiece pc = pq.q[slot];
-    if (slot >= n_init) pq.ready[slot] = 0;
-    const WalkItem it = p.walkq[pc.item];
-    const WalkView v = walk_view(p, it, true);
-    int32_t *pend = p.walk_pend + pc.item;
-    int fl = 0, ok = 0;
-    if (!(*(volatile const int32_t *)pend & WALK_FAILED)) {  // a failed sibling has already decided the walk
-        PieceFork fork{pq, pend, pc.item, n_init, false};
-        ok = stab_piece<GeomD>(v.g, v.root, (int)it.k, it.pack, v.pool, &v.cold->big, &v.cold->lock, fl, (int)pc.node, (int)pc.kind, (int)pc.skip,
-                               pc.a, pc.b, pc.c, fork);
-        if (fork.overflow) { fl |= PCT_FLAG_CAND_OVERFLOW; ok = 0; }  // never silent: the candidate stays infeasible and the env is flagged
-    }
-    if (fl) atomicOr(const_cast<int32_t *>(&v.hot->h.flags), fl);
-    if (!ok) atomicOr(pend, WALK_FAILED);
-    __threadfence();
-    const int r = atomicSub(pend, 1);
-    if ((r & (WALK_FAILED - 1)) == 1) {  // the walk's last piece
-        if (!(r & WALK_FAILED)) atomicOr(&v.cold->fbits[it.c >> 5], 1u << (it.c & 31));
-        walk_done(&v.cold->n_pending);
-    }
-    pq_piece_done(pq);
-}
-__global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_fork_kernel(const DParams p) {
-    const int lane = threadIdx.x & 31;
-    const int wid = blockIdx.x * WALK_WARPS + (threadIdx.x >> 5), n_warps = gridDim.x * WALK_WARPS;
-    const PieceQueue pq{(WalkPiece *)p.contq, p.piece_ready, p.cont_ctr, p.piece_cap};
-    const int n_init = min(*(volatile const int32_t *)(pq.ctr + PQ_NINIT), pq.cap);  // written by the light-prefix kernel only (completed)
-    const int L = p.walk_lanes;
-    pdl_launch_dependents();  // the emit kernel's blocks may become resident; each waits for ITS env's last walk
-    if (n_init > 0) {
-        // the light-prefix kernel's pieces: dealt statically
-#pragma unroll 1
-        for (int b = wid * L; b < n_init; b += n_warps * L) {
-            if (lane < L && b + lane < n_init) run_piece(p, pq, n_init, b + lane);
-            __syncwarp();
-        }
-        // forked pieces: tickets
-        const bool keep = wid < p.walk_keep;
-#pragma unroll 1
-        for (;;) {
-            int t0 = -1;
-            if (lane == 0 && (keep || *(volatile const int32_t *)(pq.ctr + PQ_ALLOC) - *(volatile const int32_t *)(pq.ctr + PQ_HEAD) > 0))
-                t0 = atomicAdd(pq.ctr + PQ_HEAD, L);
-            t0 = __shfl_sync(FULL, t0, 0);
-            if (t0 < 0) break;  // not a helper and nothing unclaimed in the queue: leave (SM slots for the emit kernel)
-            bool fin = false;
-            if (lane < L) {
-                const int slot = n_init + t0 + lane;
-                if (pq_wait(pq, slot)) run_piece(p, pq, n_init, slot);
-                else fin = true;
-            }
-            __syncwarp();
-            if (__any_sync(FULL, fin)) break;  // a lane saw the end of all work
-        }
-    }
-    if (lane == 0) pq_warp_exit(pq, n_warps, p.walk_ctr);
-}
+
+__global__ void __launch_bounds__(32 * LIGHT_WARPS, LIGHT_MINB) pct_walk_light_kernel(const DParams p) { walk_light<DWalk>(p); }
+__global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_kernel(const DParams p) { PCT_WALK_CONT_BODY(DWalk, p) }
+__global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_fork_kernel(const DParams p) { walk_fork<DWalk>(p); }
 
 constexpr int EMIT_WARPS = 4;
 constexpr int EMIT_STAGE = sizeof(DHdr) + NB_MAX * 12;  // header + placed boxes: all the observation needs from the hot record
@@ -1381,7 +1216,7 @@ __global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const DParams
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int e = blockIdx.x * EMIT_WARPS + warp;
     // last kernel of the launch sequence that touches the walk pools (both walk kernels have completed: plain stream order): empty them for the next step
-    if (blockIdx.x == 0 && threadIdx.x == 0 && p.walk_ctr && !p.walk_fork) { *p.walk_ctr = 0; p.cont_ctr[0] = 0; p.cont_ctr[1] = 0; }  // (the fork-join kernel's counters are live while this kernel starts: its last warp empties them)
+    if (blockIdx.x == 0 && threadIdx.x == 0 && p.walk.walk_ctr) reset_walk_pools(p.walk);
     if (blockIdx.x == 0 && p.order) {
         // ... and the last one of the step: the apply and candidates kernels have consumed this parity's buckets (both completed before the walk kernels
         // started) and the apply kernel has filled the other parity's; empty the consumed ones and flip
@@ -1402,14 +1237,7 @@ __global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const DParams
     if (lane == 0) {
         mbar_init(mbar, 1);
         fence_proxy_async();
-        // launched as a programmatic dependent of the continuation kernel: this block may run while walks are still in flight.  The classification
-        // (a fully completed kernel) set n_pending; the walk kernels release-decrement it after their last write of this env.
-        int spins = 0;
-        while (*(volatile const int32_t *)&cold->n_pending > 0) {
-            __nanosleep(spins < 16 ? 100 : 1000);
-            if (++spins > (1 << 22)) { atomicOr(&ghot->h.flags, PCT_FLAG_SYNC_TIMEOUT); break; }
-        }
-        __threadfence();
+        wait_walks(&cold->n_pending, ghot);
         fence_proxy_async_all();
     }
     __syncwarp();
@@ -1488,19 +1316,15 @@ template <typename OT, bool STAB, typename SlotT>
 static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
     constexpr bool BIGSM = !STAB;
     static bool attr_set = false;
-    static int n_sm = 0;
     const size_t smem1 = (size_t)K1_SM_PER_WARP * WARPS_PER_BLOCK;
     const size_t smem2 = (size_t)Lay<SlotT, BIGSM>::PER_WARP * WARPS_PER_BLOCK;
     DParams p = p_in;
-    const bool k3_old = (p.opt & PCT_OPT_K3_BLOCK) != 0 || !p.walkq;  // PCT_B200_K3=block: round 1's block-per-env / thread-per-candidate kernel (A/B measurements)
-    if (k3_old) p.walkq = nullptr;  // K2 then skips the classification
+    const bool k3_old = (p.opt & PCT_OPT_K3_BLOCK) != 0 || !p.walk.walkq;  // PCT_B200_K3=block: round 1's block-per-env / thread-per-candidate kernel (A/B measurements)
+    if (k3_old) p.walk.walkq = nullptr;  // K2 then skips the classification
     if (!attr_set) {
         cudaError_t err = set_smem(pct_apply_kernel<STAB>, smem1);
         if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB>, smem1);  // the ALIAS variant (stability settings only)
         if (err == cudaSuccess) err = set_smem(pct_candidates_kernel<SlotT, BIGSM>, smem2);
-        int dev = 0;
-        if (err == cudaSuccess) err = cudaGetDevice(&dev);
-        if (err == cudaSuccess) err = cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
         if (err != cudaSuccess) return err;
         attr_set = true;
     }
@@ -1541,8 +1365,11 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
         // the pooled walks need EVERY env's classification (plain stream order = full dependency), the emit kernel every walk
         if (p.ready && prof) cudaEventRecord(prof[2], st);
         if (STAB) {
+            int n_sm = 0;
+            err = sm_count(&n_sm);
+            if (err != cudaSuccess) return err;
             pct_walk_light_kernel<<<n_sm * LIGHT_MINB, 32 * LIGHT_WARPS, 0, st>>>(p);
-            if (p.walk_fork) pct_walk_fork_kernel<<<n_sm * max(1, min(p.walk_blocks, WALK_MINB)), 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
+            if (p.walk.walk_fork) pct_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, WALK_MINB)), 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
             else pct_walk_kernel<<<n_sm * WALK_MINB, 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave (every block starts at once: the emit kernel may follow)
         }
         const int eb = (p.n_envs + EMIT_WARPS - 1) / EMIT_WARPS;
@@ -1568,7 +1395,7 @@ static cudaError_t launch_s(const DParams &p, cudaStream_t st, cudaEvent_t *prof
 
 // number of kernels one reset / step enqueues (for pct_kernel_launches): apply, candidates (+ classify), [walk], emit, order / pool reset
 int discrete_kernels_per_step(const DParams &p) {
-    if ((p.opt & PCT_OPT_K3_BLOCK) || !p.walkq) return 3;
+    if ((p.opt & PCT_OPT_K3_BLOCK) || !p.walk.walkq) return 3;
     return 3 + (p.setting != 2 ? 2 : 0);
 }
 

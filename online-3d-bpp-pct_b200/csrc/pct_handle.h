@@ -15,7 +15,6 @@ struct pct_env_batch {
     pct::DEnvHot *d_hot = nullptr;
     pct::DEnvCold *d_cold = nullptr;
     void *c_state = nullptr;  // continuous-domain state (pct_continuous.cu)
-    void *c_walkq = nullptr;  // continuous-domain pool of stability walks (WalkItemC, pct_continuous.cu)
     double *d_item_set = nullptr;
     int n_items = 0;
     double *d_stream = nullptr;
@@ -56,10 +55,11 @@ struct pct_env_batch {
     cudaStream_t own_stream = nullptr;
     void *dbg = nullptr;
     int32_t *d_order = nullptr;   // heaviest-first scheduling order: parity, bucket counts, per-bucket env lists (pct_discrete.cu order_lookup)
-    pct::WalkItem *d_walkq = nullptr;  // [n_envs * CAND_MAX] pool of stability walks of the current step (pct_walk_kernel)
+    // pooled stability walks (pct_walks.cuh), both domains: create_walk_pools / walk_pools
+    void *d_walkq = nullptr;           // [n_envs * CAND_MAX] pool of stability walks of the current step (WalkItem / WalkItemC)
     int32_t *d_walk_ctr = nullptr;     // [n_envs] fill counters (index = first env of the launched range)
-    pct::WalkCont *d_contq = nullptr;  // [n_envs * WALK_CONT_PER_ENV] continuations: light-prefix kernel -> pct_walk_kernel
-    int32_t *d_cont_ctr = nullptr;
+    pct::WalkCont *d_contq = nullptr;  // [n_envs * WALK_CONT_PER_ENV] continuations: light-prefix kernel -> continuation kernel
+    int32_t *d_cont_ctr = nullptr;     // [8 * (n_envs + 1)] eight counters per (possible) env range
     size_t contq_env_bytes = 0;        // bytes of d_contq per env (WalkCont pool / WalkPiece queue)
     int32_t *d_piece_ready = nullptr, *d_walk_pend = nullptr;  // fork-join walks: per-slot publication flags, per-walk piece counters
     bool walk_fork = false;            // PCT_B200_WALK=fork: fork-join continuation kernel (pct_walkq.cuh) instead of the sequential one — measured equal-to-slower (DESIGN.md section 5), kept as an opt-in
@@ -77,3 +77,22 @@ struct pct_env_batch {
     cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
 };
 
+namespace pct {
+// allocates the pools of the stability walks with queue entries of `item_bytes` (pct_create, continuous_create; not with PCT_B200_K3=block)
+cudaError_t create_walk_pools(pct_env_batch *h, size_t item_bytes);
+
+// the pools of the env range [off, off + cnt): env ranges stepped concurrently (pct_step_host's staged path) own disjoint slices
+template <typename Item>
+WalkPools<Item> walk_pools(const pct_env_batch *h, int off, int cnt) {
+    WalkPools<Item> w{};
+    w.walkq = h->d_walkq ? (Item *)h->d_walkq + (size_t)off * CAND_MAX : nullptr;
+    w.walk_ctr = h->d_walk_ctr ? h->d_walk_ctr + off : nullptr;
+    w.contq = h->d_contq ? (WalkCont *)((char *)h->d_contq + (size_t)off * h->contq_env_bytes) : nullptr;
+    w.cont_ctr = h->d_cont_ctr ? h->d_cont_ctr + 8 * (size_t)off : nullptr;
+    w.walk_lanes = h->walk_lanes; w.walk_lanes_tall = h->walk_lanes_tall;
+    w.walk_fork = h->walk_fork ? 1 : 0; w.walk_blocks = h->walk_blocks; w.walk_keep = h->walk_keep; w.piece_cap = cnt * WALK_PIECES_PER_ENV;
+    w.piece_ready = h->d_piece_ready ? h->d_piece_ready + (size_t)off * WALK_PIECES_PER_ENV : nullptr;
+    w.walk_pend = h->d_walk_pend ? h->d_walk_pend + (size_t)off * CAND_MAX : nullptr;
+    return w;
+}
+}  // namespace pct

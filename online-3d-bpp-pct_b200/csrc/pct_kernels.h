@@ -1,5 +1,6 @@
 // Internal: device record layouts and kernel launch parameters shared by the kernels and the C-ABI layer.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "pct_b200.h"
@@ -175,6 +176,26 @@ constexpr int WALK_FAILED = 1 << 30;
 constexpr int WALK_PIECES_PER_ENV = 1024;  // capacity of the fork-join piece queue = n_envs x this (32 B entries; mean use ~5 per env); overflow -> PCT_FLAG_CAND_OVERFLOW
 constexpr int WALK_CONT_PER_ENV = 256;  // capacity of the continuation pool = n_envs x this (mean use: 3 per env); overflow -> PCT_FLAG_CAND_OVERFLOW
 
+// The pooled stability walks of one launch (pct_walks.cuh), the same for both domains but for the queue entry (WalkItem / WalkItemC).  Embedded in
+// DParams and CParams where the fields stood one by one: the static_asserts behind each struct pin the byte offsets the kernels' code depends on.
+template <typename Item>
+struct WalkPools {
+    Item *walkq;        // [n_envs * CAND_MAX] the step's pool of stability walks (worst-case capacity; only the used prefix is touched); nullptr: round 1's block kernel
+    int32_t *walk_ctr;  // its fill counter; reset by the emit kernel (sequential walks) / the last warp of the fork-join kernel
+    WalkCont *contq;    // [n_envs * WALK_CONT_PER_ENV] walks the light-prefix kernel hands to the continuation kernel
+    int32_t *cont_ctr;  // [2]: continuations pooled from the front (ordinary) / from the end (tall walks) of contq
+    int32_t walk_lanes, walk_lanes_tall; // continuations per warp of the continuation kernel (1..32): ordinary / tall (resting height >= 0.6 H) walks
+    // fork-join walks (pct_walk_fork_kernel, opt-in with PCT_B200_WALK=fork; the default is the sequential continuation kernel): contq holds WalkPiece entries,
+    // cont_ctr = the queue's counters (pct_walkq.cuh); piece_ready[slot] = 1 once the slot's piece is written (cleared by its consumer);
+    // walk_pend[item] = pieces of the walk still running (+ WALK_FAILED once one of them failed)
+    int32_t walk_fork;
+    int32_t walk_blocks;   // blocks per SM of the fork-join kernel (1..8)
+    int32_t walk_keep;     // its warps that stay as helpers for forked pieces until the step's walks are done (the others leave when the fork queue is empty)
+    int32_t piece_cap;     // entries of contq / piece_ready in this launch (WALK_PIECES_PER_ENV per env)
+    int32_t *piece_ready;
+    int32_t *walk_pend;
+};
+
 struct DParams {
     DEnvHot *hot;
     DEnvCold *cold;
@@ -213,22 +234,11 @@ struct DParams {
     int32_t *order;  // heaviest-first scheduling order of the apply / candidates kernels: parity, bucket counts, per-bucket env lists (pct_discrete.cu, order_lookup); nullptr = env order
     int32_t *ready;  // [2 * n_envs] per-env hand-over flags (apply -> candidates, candidates -> feas_emit); nullptr = kernels run back to back
     int32_t epoch;   // value published in `ready` by this launch
-    WalkItem *walkq;    // [n_envs * CAND_MAX] the step's pool of stability walks (worst-case capacity; only the used prefix is touched)
-    int32_t *walk_ctr;  // its fill counter; reset by the emit kernel (sequential walks) / the last warp of the fork-join kernel
-    WalkCont *contq;    // [n_envs * WALK_CONT_PER_ENV] walks the light-prefix kernel hands to the continuation kernel
-    int32_t *cont_ctr;  // [2]: continuations pooled from the front (ordinary) / from the end (tall walks) of contq
-    int32_t walk_lanes, walk_lanes_tall; // continuations per warp of pct_walk_kernel (1..32): ordinary / tall (resting height >= 0.6 H) walks
-    // fork-join walks (pct_walk_fork_kernel, opt-in with PCT_B200_WALK=fork; the default is the sequential continuation kernel): contq holds WalkPiece entries,
-    // cont_ctr = the queue's counters (pct_walkq.cuh); piece_ready[slot] = 1 once the slot's piece is written (cleared by its consumer);
-    // walk_pend[item] = pieces of the walk still running (+ WALK_FAILED once one of them failed)
-    int32_t walk_fork;
-    int32_t walk_blocks;   // blocks per SM of the fork-join kernel (1..8)
-    int32_t walk_keep;     // its warps that stay as helpers for forked pieces until the step's walks are done (the others leave when the fork queue is empty)
-    int32_t piece_cap;     // entries of contq / piece_ready in this launch (WALK_PIECES_PER_ENV per env)
-    int32_t *piece_ready;
-    int32_t *walk_pend;
+    WalkPools<WalkItem> walk;
     int32_t opt;     // opt-in variants served by `aux`: PCT_OPT_DELTA (K3 delta observation writes), PCT_OPT_ALIAS (K1 object semantics of the loads)
 };
+static_assert(sizeof(WalkPools<WalkItem>) == 72 && offsetof(DParams, walk) == 240 && offsetof(DParams, opt) == 312 && sizeof(DParams) == 320,
+              "walk pools at the byte offsets of the fields they replaced");
 constexpr int PCT_OPT_DELTA = 1, PCT_OPT_ALIAS = 2, PCT_OPT_K3_BLOCK = 4, PCT_OPT_NO_EMIT_PDL = 8;  // K3_BLOCK: round 1's block-per-env feasibility kernel (A/B)
 
 // heuristic baselines (pct_heuristics.cuh)
@@ -299,6 +309,9 @@ struct PreKernel {
 
 // delta observation writes: aux[i].obs_prev = {nb, nl} for n envs ("every row of the buffer may be non-zero")
 void launch_fill_prev(DEnvAux *aux, int n_envs, int nb, int nl, cudaStream_t st);
+
+// multiprocessors of the current device, looked up once: the walk kernels launch one resident wave of blocks
+cudaError_t sm_count(int *n);
 
 int discrete_kernels_per_step(const DParams &p);
 // apply = false: the sequence without the apply kernel (pct_set_items / pct_reset_envs; p.ready and p.order must be nullptr)
