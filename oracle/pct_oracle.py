@@ -39,7 +39,7 @@ def lib():
         L.pcto_get_ems.argtypes = [C.c_void_p, ip, C.c_int]
         L.pcto_get_candidates.argtypes = [C.c_void_p, ip, ip, C.c_int]
         L.pcto_get_packed.argtypes = [C.c_void_p, ip, C.c_int]
-        for f in ("pcto_n_lstsq", "pcto_n_boxes", "pcto_stream_pos"):
+        for f in ("pcto_n_lstsq", "pcto_n_boxes", "pcto_stream_pos", "pcto_n_ems_intermediate", "pcto_n_raw_candidates", "pctc_n_ems_intermediate"):
             getattr(L, f).argtypes = [C.c_void_p]
         L.pcto_set_order6.argtypes = [C.POINTER(C.c_int64), C.c_int, ip]
         L.pcto_hull_shrunk.argtypes = [dp, C.c_int, dp]
@@ -133,6 +133,14 @@ class OracleDiscrete(object):
         feas = np.zeros(8192, dtype=np.int32)
         n = self.L.pcto_get_candidates(self.h, _ip(buf), _ip(feas), 8192)
         return buf[:n].copy(), feas[:n].copy()
+
+    def n_ems_intermediate(self):
+        """length of the last placement's GENEMS list before EliminateInscribedEMS (survivors + children; 0 after a reset)"""
+        return self.L.pcto_n_ems_intermediate(self.h)
+
+    def n_raw_candidates(self):
+        """length of the insertion sequence the last candidate generator fed to the set, before it dedupes it"""
+        return self.L.pcto_n_raw_candidates(self.h)
 
     @property
     def packed(self):
@@ -377,6 +385,10 @@ class OracleContinuous(object):
         feas = np.zeros(8192, dtype=np.int32)
         n = self.L.pctc_get_candidates(self.h, _dp(buf), _ip(feas), 8192)
         return buf[:n].copy(), feas[:n].copy()
+
+    def n_ems_intermediate(self):
+        """length of the last placement's GENEMS list before EliminateInscribedEMS (survivors + children; 0 after a reset)"""
+        return self.L.pctc_n_ems_intermediate(self.h)
 
     @property
     def packed(self):

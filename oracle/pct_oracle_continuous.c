@@ -59,6 +59,7 @@ typedef struct pctc_env {
     double next_den;
     int error, n_lstsq;
     int last_ncand;
+    int last_ntmp; /* length of the last GENEMS intermediate list (survivors + children, before EliminateInscribedEMS) */
     double last_cand[PC_MAX_CAND][6];
     int last_feas[PC_MAX_CAND];
     int n_packed;
@@ -353,6 +354,7 @@ static void genems(pctc_env *e, const double loc[6]) {
         e->n_ems = w;
     }
     free(del);
+    e->last_ntmp = e->n_ems;
     int n = e->n_ems;
     char *df = calloc(n + 1, 1);
     for (int i = 0; i < n; i++)
@@ -525,6 +527,7 @@ void pctc_reset(pctc_env *e, double *obs) {
     e->ems[0][0] = e->ems[0][1] = e->ems[0][2] = 0; e->ems[0][3] = e->W; e->ems[0][4] = e->L; e->ems[0][5] = e->H;
     e->n_boxes = 0;
     e->error = 0;
+    e->last_ntmp = 0;
     creator_generate(e);
     cur_observation(e, obs);
 }
@@ -586,6 +589,7 @@ int pctc_get_candidates(pctc_env *e, double *out6, int *feas, int cap) {
 }
 int pctc_get_packed(pctc_env *e, double *out7, int cap) { int n = e->n_packed < cap ? e->n_packed : cap; memcpy(out7, e->packed, sizeof(double[7]) * n); return e->n_packed; }
 int pctc_n_lstsq(pctc_env *e) { return e->n_lstsq; }
+int pctc_n_ems_intermediate(pctc_env *e) { return e->last_ntmp; }
 
 /* What heuristic.py reads from a PackingContinuous env (heuristic.py:163-166,190-193,387-416,541-567):
  * Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) (C:space.py:380-425; max_h is

@@ -81,6 +81,85 @@ def cont_case_stream(c, seed, env, n):
     return s
 
 
+# ---- fixed capacities of the step kernels (include/pct_b200.h flags; DESIGN.md section 7) ----------------------------------
+# name -> (flag bit, capacity).  Every count the oracle reports is compared with its capacity: a count above it must flag.
+FLAG_BOX, FLAG_EMS, FLAG_CAND = 1, 4, 8
+CAPS = {
+    "discrete": {"ems": (FLAG_EMS, 128), "ems_tmp": (FLAG_EMS, 256), "cand": (FLAG_CAND, 1228), "raw": (FLAG_CAND, 2048)},
+    "continuous": {"ems": (FLAG_EMS, 256), "ems_tmp": (FLAG_EMS, 512), "cand": (FLAG_CAND, 1228)},
+}
+
+
+def load_capacity_cases():
+    """name -> case dict of tests/golden/capacity_cases.npz (tests/golden/make_capacity_cases.py), its item stream under 'stream'"""
+    import json
+    import os
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "capacity_cases.npz"))
+    out = {}
+    for c in json.loads(str(z["meta"])):
+        c.update(stream=z[c["name"]], container=tuple(c["container"]))
+        out[c["name"]] = c
+    return out
+
+
+def capacity_oracle(c):
+    """oracle env of a capacity case (tests/golden/capacity_cases.npz)"""
+    from pct_oracle import OracleContinuous
+    if c["domain"] == "continuous":
+        return OracleContinuous(c["setting"], container_size=c["container"], internal_node_holder=c["nb"], leaf_node_holder=c["nl"],
+                                size_minimum=c["size_minimum"], stream=c["stream"])
+    return OracleDiscrete(c["setting"], container_size=c["container"], internal_node_holder=c["nb"], leaf_node_holder=c["nl"],
+                          size_minimum=c["size_minimum"], stream=c["stream"], lnes=c.get("lnes", "EMS"))
+
+
+def oracle_counts(orc, lnes="EMS"):
+    """the oracle's list lengths after its last reset / step, by capacity name"""
+    d = {"ems": len(orc.ems()), "ems_tmp": orc.n_ems_intermediate(), "cand": len(orc.candidates()[0])}
+    if isinstance(orc, OracleDiscrete) and lnes in ("EP", "CP", "FC"):
+        d["raw"] = orc.n_raw_candidates()
+    return d
+
+
+def expected_flags(c, counts, step_info):
+    """flag bits the kernels must raise on a step whose oracle counts / info are these"""
+    f = 0
+    for name, (bit, cap) in CAPS[c["domain"]].items():
+        if counts.get(name, 0) > cap:
+            f |= bit
+    if step_info.get("error") == 1:  # more boxes than internal_node_holder: IndexError in the reference
+        f |= FLAG_BOX
+    return f
+
+
+def capacity_trace(c):
+    """Replay a capacity case on the oracle with the shared policy (env 0 of seed c['pseed']), for at most c['steps'] steps, up to the
+    first step that ends the episode or must flag.  -> dict: reset_flags (flags the reset's counts call for), n_steps (steps run),
+    t_star (index of the first step that must flag, -1: none), flag (its bits), done (the last step ended the episode),
+    peak (largest count per name and box count over the reset and every step before t_star)."""
+    orc = capacity_oracle(c)
+    lnes = c.get("lnes", "EMS")
+    obs = orc.reset()
+    cnt = oracle_counts(orc, lnes)
+    peak = dict(cnt, boxes=0)
+    out = dict(reset_flags=expected_flags(c, cnt, {}), n_steps=0, t_star=-1, flag=0, done=False)
+    for t in range(c["steps"]):
+        _, row = policy_pick(obs, c["nb"], c["nl"], c["pseed"], 0, t)
+        obs, _, done, info = orc.step(row)
+        cnt = oracle_counts(orc, lnes)
+        f = expected_flags(c, cnt, info)
+        out.update(n_steps=t + 1, done=bool(done))
+        if f:
+            out.update(t_star=t, flag=f, star=cnt)
+            break
+        for k, v in cnt.items():
+            peak[k] = max(peak[k], v)
+        peak["boxes"] = max(peak["boxes"], len(orc.packed))
+        if done:
+            break
+    out["peak"] = peak
+    return out
+
+
 class OracleVec(object):
     """N independent oracle envs with the ShmemVecEnv worker semantics (auto-reset on done,
     wrapper/shmem_vec_env.py:139-143) and the shared deterministic policy."""
