@@ -115,6 +115,30 @@ typedef struct pct_state_dump {
     double ems[256][6];
 } pct_state_dump;
 
+/* Host-side dump of the support graph one environment carries from step to step in the stability settings (parity tests): what the
+ * real placements' stability descents wrote and every later feasibility walk reads.  Slot-independent: box indices are placement
+ * order, list positions are gone.  Box index n_box stands for the box of a FAILED real placement (its loads stay on its supports
+ * until the env resets, as the reference's up_edges keep them).
+ *   supports of placed box u : sup[sup_off[u] .. sup_off[u+1])                 (stored order = scan order at its placement)
+ *   loads resting on box t   : rows load_off[t] .. load_off[t+1]              (insertion order of the reference's up_edges dict)
+ *     load_upper = the box the load comes from, load = centre x, y, z and mass as the read-only walks read them,
+ *     load_alias = 1: the entry is the upper box's own stack object (alias mode only, else 0)
+ *   stored support polygon of box u : poly[poly_off[u] .. poly_off[u+1]) (shrunk hull vertices; only boxes with >= 2 supports store
+ *     one, none when the polygon pool had no room), poly_pos[u] = its position in the pool; with exactly two supports
+ *     has_split[u] = 1 and split[u] = the stored split direction
+ *   own_stack[u] : the box's own stack (centre x, y, z, mass), alias mode only; defined for boxes with a support or a load
+ *   alias_stale : alias bits at or beyond n_edge (left by earlier episodes; every new edge rewrites its bit) */
+typedef struct pct_support_graph {
+    int32_t n_box, n_edge, n_poly, alias;
+    int32_t alias_stale, pad_;
+    int32_t sup_off[82], load_off[82], poly_off[82], poly_pos[82], has_split[82];
+    int32_t sup[256], load_upper[256], load_alias[256];
+    double load[256][4];
+    double poly[256][2];
+    double split[82][2];
+    double own_stack[82][4];
+} pct_support_graph;
+
 /* gym.make('PctDiscrete-v0' | 'PctContinuous-v0', **kwargs) x n_envs   (envs.py:84-108, tools.py:232-240) */
 int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle *out);
 /* VecEnv.close()  (wrapper/vec_env.py:93-99) */
@@ -308,6 +332,10 @@ int pct_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_
 
 /* introspection */
 int pct_get_state(pct_handle h, int32_t env, pct_state_dump *out);
+/* Same contract as pct_get_state (synchronises the device, copies the env's records to the host, decodes there; no kernel), both
+ * domains, both alias modes; setting 2 keeps no graph and yields the empty one.  The stored lists are walked defensively: a cycle, an
+ * index beyond n_edge / n_box or an edge filed in two lists returns PCT_ERR_STATE with the finding in pct_last_error. */
+int pct_get_support_graph(pct_handle h, int32_t env, pct_support_graph *out);
 int32_t pct_obs_len(pct_handle h);       /* (NB + NL + 1) * 9 */
 int32_t pct_num_envs(pct_handle h);
 int64_t pct_state_bytes_per_env(pct_handle h); /* HBM bytes of library-owned state per env (roofline accounting) */

@@ -38,12 +38,35 @@ class StateDump(C.Structure):
                 ("boxes", (C.c_double * 7) * 80), ("ems", (C.c_double * 6) * 256)]
 
 
+class SupportGraph(C.Structure):
+    _fields_ = [("n_box", C.c_int32), ("n_edge", C.c_int32), ("n_poly", C.c_int32), ("alias", C.c_int32), ("alias_stale", C.c_int32), ("pad_", C.c_int32),
+                ("sup_off", C.c_int32 * 82), ("load_off", C.c_int32 * 82), ("poly_off", C.c_int32 * 82), ("poly_pos", C.c_int32 * 82),
+                ("has_split", C.c_int32 * 82), ("sup", C.c_int32 * 256), ("load_upper", C.c_int32 * 256), ("load_alias", C.c_int32 * 256),
+                ("load", (C.c_double * 4) * 256), ("poly", (C.c_double * 2) * 256), ("split", (C.c_double * 2) * 82),
+                ("own_stack", (C.c_double * 4) * 82)]
+
+
+def graph_to_dict(d):
+    """pct_support_graph -> the canonical per-env form (tests/harness.py): lists per placed box, floats as numpy float64"""
+    import numpy as np
+    f = lambda name: np.ctypeslib.as_array(getattr(d, name)).copy()
+    nb = d.n_box
+    so, lo, po = f("sup_off"), f("load_off"), f("poly_off")
+    sup, up, al, load, poly, split, own = f("sup"), f("load_upper"), f("load_alias"), f("load"), f("poly"), f("split"), f("own_stack")
+    return dict(n_box=nb, n_edge=d.n_edge, n_poly=d.n_poly, alias=bool(d.alias), alias_stale=d.alias_stale,
+                supports=[sup[so[u]:so[u + 1]].tolist() for u in range(nb)],
+                load_upper=[up[lo[u]:lo[u + 1]].tolist() for u in range(nb)], load_alias=[al[lo[u]:lo[u + 1]].tolist() for u in range(nb)],
+                loads=[load[lo[u]:lo[u + 1]] for u in range(nb)], polygon=[poly[po[u]:po[u + 1]] for u in range(nb)],
+                poly_pos=f("poly_pos")[:nb].tolist(), split=[split[u] if d.has_split[u] else None for u in range(nb)],
+                own_stack=own[:nb] if d.alias else None)
+
+
 EXPORTS = ["pct_create", "pct_destroy", "pct_last_error", "pct_set_item_set", "pct_set_item_stream", "pct_set_trajectory_length", "pct_reset", "pct_step",
            "pct_step_host", "pct_reset_host", "pct_policy_random", "pct_policy_random_dev", "pct_get_state", "pct_obs_len", "pct_num_envs",
            "pct_state_bytes_per_env", "pct_kernel_launches", "pct_version", "pct_profile_enable", "pct_profile_read", "pct_heuristic_actions",
            "pct_heuristic_actions_f64", "pct_query_placement", "pct_query_placement_f64",
            "pct_snapshot_bytes", "pct_snapshot", "pct_restore", "pct_query_placements", "pct_query_placements_f64", "pct_height_maps",
-           "pct_preview_items", "pct_set_items", "pct_reset_envs"]
+           "pct_preview_items", "pct_set_items", "pct_reset_envs", "pct_get_support_graph"]
 
 
 def build(verbose=False):
@@ -79,6 +102,7 @@ def lib():
     L.pct_policy_random.argtypes = [vp, vp, u64, i64, vp]
     L.pct_policy_random_dev.argtypes = [vp, vp, u64, vp, vp]
     L.pct_get_state.argtypes = [vp, i32, C.POINTER(StateDump)]
+    L.pct_get_support_graph.argtypes = [vp, i32, C.POINTER(SupportGraph)]
     L.pct_obs_len.argtypes = [vp]
     L.pct_num_envs.argtypes = [vp]
     L.pct_state_bytes_per_env.argtypes = [vp]

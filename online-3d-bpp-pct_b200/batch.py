@@ -439,6 +439,13 @@ class PctBatch(object):
         return dict(n_boxes=d.n_boxes, n_ems=d.n_ems, n_leaf=d.n_leaf, flags=d.flags, draw_pos=d.draw_pos,
                     next_box=list(d.next_box), next_den=d.next_den, boxes=boxes, ems=ems)
 
+    def support_graph(self, env):
+        """The support graph env `env` carries between steps (pct_get_support_graph): per placed box its supports, the loads resting on it
+        in insertion order, its stored support polygon and, in the alias mode, its own stack.  Synchronises; for parity tests."""
+        d = _lib.SupportGraph()
+        self._check(self.L.pct_get_support_graph(self.h, int(env), C.byref(d)), "pct_get_support_graph")
+        return _lib.graph_to_dict(d)
+
     def profile(self, on=True):
         self._check(self.L.pct_profile_enable(self.h, int(on)), "pct_profile_enable")
 

@@ -8,11 +8,13 @@
 
 #include "pct_kernels.h"
 #include "pct_handle.h"
+#include "pct_support_graph.h"
 
 using namespace pct;
 
 static thread_local std::string g_create_err;
-static_assert(sizeof(pct_config) == 112 && sizeof(pct_step_info) == 32, "C ABI layout (tests/test_cabi.py checks the ctypes mirror against the same numbers)");
+static_assert(sizeof(pct_config) == 112 && sizeof(pct_step_info) == 32 && sizeof(pct_support_graph) == 20960,
+              "C ABI layout (tests/test_cabi.py checks the ctypes mirror against the same numbers)");
 
 #define CK(h, call)                                                                                        \
     do {                                                                                                   \
@@ -32,6 +34,7 @@ int continuous_launch(pct_env_batch *h, int mode, const void *actions, int actio
 int continuous_preview(pct_env_batch *h, const ItemParams &ip, cudaStream_t st);
 int continuous_policy_random(pct_env_batch *h, int32_t *leaf_idx, uint64_t seed, int64_t t, cudaStream_t st);
 int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out);
+int continuous_get_support_graph(pct_env_batch *h, int env, const DEnvAux *aux, pct_support_graph *out, char *err, size_t cap);
 int64_t continuous_state_bytes();
 int continuous_heuristic(pct_env_batch *h, int code, double *rows, double *hstate, cudaStream_t st);
 int continuous_query(pct_env_batch *h, int env, const double q[5], double density, double *d_out, cudaStream_t st);
@@ -717,6 +720,36 @@ int pct_get_state(pct_handle h, int32_t env, pct_state_dump *out) {
     }
     for (int i = 0; i < hot.h.n_ems && i < 256 && i < E_MAX; i++)
         for (int t = 0; t < 6; t++) out->ems[i][t] = hot.ems[i][t];
+    return PCT_OK;
+}
+
+int pct_get_support_graph(pct_handle h, int32_t env, pct_support_graph *out) {
+    if (!h || !out || env < 0 || env >= h->n_envs) return PCT_ERR_INVALID;
+    CK(h, cudaSetDevice(h->device));
+    CK(h, cudaDeviceSynchronize());
+    std::vector<DEnvAux> aux(1);
+    const bool alias = h->cfg.setting != 2 && h->alias_mode && h->d_aux;
+    if (alias) CK(h, cudaMemcpy(aux.data(), h->d_aux + env, sizeof(DEnvAux), cudaMemcpyDeviceToHost));
+    char err[256] = "";
+    bool ok;
+    if (h->cfg.domain == PCT_CONTINUOUS) {
+        const int rc = continuous_get_support_graph(h, env, alias ? aux.data() : nullptr, out, err, sizeof err);
+        if (rc != PCT_OK && rc != PCT_ERR_STATE) { h->err = "pct_get_support_graph: copy of the env record failed"; return rc; }
+        ok = rc == PCT_OK;
+    } else {
+        std::vector<DEnvHot> hot(1);
+        std::vector<Stack4> st(EDGE_MAX + 1);
+        std::vector<double> poly(2 * POLY_MAX);
+        CK(h, cudaMemcpy(hot.data(), h->d_hot + env, sizeof(DEnvHot), cudaMemcpyDeviceToHost));
+        CK(h, cudaMemcpy(st.data(), (const char *)(h->d_cold + env) + offsetof(DEnvCold, e_st), sizeof(Stack4) * (EDGE_MAX + 1), cudaMemcpyDeviceToHost));
+        CK(h, cudaMemcpy(poly.data(), (const char *)(h->d_cold + env) + offsetof(DEnvCold, poly), sizeof(double) * 2 * POLY_MAX, cudaMemcpyDeviceToHost));
+        const DEnvHot &e = hot[0];
+        if (h->cfg.setting == 2) { memset(out, 0, sizeof *out); out->n_box = e.h.n_box; return PCT_OK; }
+        const GraphRecord r{e.h.n_box, e.h.n_edge, e.h.n_poly, e.e_off, e.poly_off, e.e_lower, e.e_next, e.first_in, e.last_in, st.data(), poly.data(),
+                            alias ? aux[0].box_st : nullptr, alias ? aux[0].e_upper : nullptr, alias ? aux[0].e_alias : nullptr};
+        ok = decode_support_graph(r, out, err, sizeof err);
+    }
+    if (!ok) { h->err = "pct_get_support_graph: env " + std::to_string(env) + ": " + err; return PCT_ERR_STATE; }
     return PCT_OK;
 }
 

@@ -17,6 +17,7 @@
 #include "pct_geom_continuous.cuh"
 #include "pct_walks.cuh"
 #include "pct_continuous.cuh"
+#include "pct_support_graph.h"
 
 namespace pct {
 
@@ -283,7 +284,7 @@ __global__ void __launch_bounds__(64) pctc_apply_kernel(const CParams p) {
         // ---- Space.drop_box (C:space.py:329-376) ----
         bool ok = !(lx + x - 1e-6 > p.W || ly + y - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
         double max_h = 0;
-        if (lane == 0) { ev->e_off[n_box0] = (uint16_t)h.n_edge; ev->poly_off[n_box0] = (uint16_t)h.n_poly; ev->first_in[n_box0 < NB_MAX ? n_box0 : 0] = EDGE_NIL; }
+        if (lane == 0) { ev->e_off[n_box0] = (uint16_t)h.n_edge; ev->poly_off[n_box0] = (uint16_t)h.n_poly; if (n_box0 < NB_MAX) ev->first_in[n_box0] = EDGE_NIL; }
         __syncwarp();
         if (ok) {
             double mh = rest_height_c(ev->box, lane, n_box0, 32, lx, ly, lx + x, ly + y);
@@ -1056,6 +1057,20 @@ int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out) {
         for (int t = 0; t < 6; t++) out->ems[i][t] = tmp->ems[i][t];
     free(tmp);
     return PCT_OK;
+}
+
+int continuous_get_support_graph(pct_env_batch *h, int env, const DEnvAux *aux, pct_support_graph *out, char *err, size_t cap) {
+    CEnv *tmp = (CEnv *)malloc(sizeof(CEnv));
+    if (cudaMemcpy(tmp, (CEnv *)h->c_state + env, sizeof(CEnv), cudaMemcpyDeviceToHost) != cudaSuccess) { free(tmp); return PCT_ERR_CUDA; }
+    bool ok = true;
+    if (h->cfg.setting == 2) { memset(out, 0, sizeof *out); out->n_box = tmp->h.n_box; }
+    else {
+        const GraphRecord r{tmp->h.n_box, tmp->h.n_edge, tmp->h.n_poly, tmp->e_off, tmp->poly_off, tmp->e_lower, tmp->e_next, tmp->first_in, tmp->last_in,
+                            tmp->e_st, &tmp->poly[0][0], aux ? aux->box_st : nullptr, aux ? aux->e_upper : nullptr, aux ? aux->e_alias : nullptr};
+        ok = decode_support_graph(r, out, err, cap);
+    }
+    free(tmp);
+    return ok ? PCT_OK : PCT_ERR_STATE;
 }
 
 }  // namespace pct

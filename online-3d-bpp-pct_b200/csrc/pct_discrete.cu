@@ -778,7 +778,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kerne
         if (STAB && lane == 0) {  // CSR slot / incoming-list head of the box about to be placed
             hot->e_off[n_box0] = (uint16_t)h.n_edge;
             hot->poly_off[n_box0] = (uint16_t)h.n_poly;
-            hot->first_in[n_box0 < NB_MAX ? n_box0 : 0] = EDGE_NIL;
+            if (n_box0 < NB_MAX) hot->first_in[n_box0] = EDGE_NIL;  // box NB_MAX + 1 is never committed and nothing rests on a box during its own descent
         }
         __syncwarp();
         if (ok) {

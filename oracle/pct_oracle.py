@@ -59,6 +59,25 @@ def _ip(a):
     return a.ctypes.data_as(C.POINTER(C.c_int))
 
 
+def _support_graph(fn, h):
+    """the env's support graph in the canonical form of tests/harness.py (read-only export, PO_DEFINE_GET_SUPPORT_GRAPH)"""
+    ce, cp = 8192, 32768
+    hdr = np.zeros(6, dtype=np.int32)
+    so, lo, po = (np.zeros(258, dtype=np.int32) for _ in range(3))
+    sup, up, al = (np.zeros(ce, dtype=np.int32) for _ in range(3))
+    c2d, load, poly, own = np.zeros((ce, 2)), np.zeros((ce, 4)), np.zeros((cp, 2)), np.zeros((257, 4))
+    fn.argtypes = [C.c_void_p] + [C.c_void_p] * 11 + [C.c_int, C.c_int]
+    rc = fn(h, *[a.ctypes.data for a in (hdr, so, sup, c2d, lo, up, al, load, po, poly, own)], ce, cp)
+    if rc:
+        raise RuntimeError("oracle support graph export failed (an up_edges key of no box, or more entries than the export holds)")
+    nb = int(hdr[0])
+    return dict(n_box=nb, n_edge=int(hdr[1]), alias=bool(hdr[5]), failed_box=(bool(hdr[2]), int(hdr[3]), int(hdr[4])),
+                supports=[sup[so[u]:so[u + 1]].tolist() for u in range(nb)], c2d=[c2d[so[u]:so[u + 1]].copy() for u in range(nb)],
+                load_upper=[up[lo[u]:lo[u + 1]].tolist() for u in range(nb)], load_alias=[al[lo[u]:lo[u + 1]].tolist() for u in range(nb)],
+                loads=[load[lo[u]:lo[u + 1]].copy() for u in range(nb)], polygon=[poly[po[u]:po[u + 1]].copy() for u in range(nb)],
+                own_stack=own[:nb].copy())
+
+
 class OracleDiscrete(object):
     """Single discrete env, same call surface as the reference's PackingDiscrete
     (pct_envs/PctDiscrete0/bin3D.py:8-188) restricted to LNES='EMS', shuffle=False and an injected
@@ -182,6 +201,9 @@ class OracleDiscrete(object):
     @property
     def stream_pos(self):
         return self.L.pcto_stream_pos(self.h)
+
+    def support_graph(self):
+        return _support_graph(self.L.pcto_get_support_graph, self.h)
 
     def __del__(self):
         try:
@@ -418,6 +440,9 @@ class OracleContinuous(object):
     @property
     def n_lstsq(self):
         return self.L.pctc_n_lstsq(self.h)
+
+    def support_graph(self):
+        return _support_graph(self.L.pctc_get_support_graph, self.h)
 
     def __del__(self):
         try:

@@ -393,4 +393,41 @@ static int po_pyset_order(const po_pyset *s, int *out) {
     return m;
 }
 
+/* ---- read-only export of the support graph an env keeps between steps (tests/harness.py "canonical support graph") ----------------
+ * Both env types share the field names used here.  Per placed box u, in placement order:
+ *   supports  be_box (bottom_edges order) with the contact centres c2d;   loads  up_edges in dict order: the upper box's placement index
+ *   (n_boxes = the box whose real placement failed: its entries stay in the dicts and, found under no live box, keep their last value),
+ *   the value calculate_new_com reads for the entry (the live stack of the upper box in alias mode, else the stored one), its alias bit;
+ *   polygon  bottom_whole_contact_area;   own  thisStack.
+ * hdr = {n_boxes, number of up_edges entries, the failed box has entries, its number of supports, its polygon length, alias_mode}.
+ * Returns 0, or -1 when a caller array (cap_e edges, cap_p vertices) is too small / an entry's key belongs to no box. */
+#define PO_DEFINE_GET_SUPPORT_GRAPH(fname, env_t, max_boxes)                                                                          \
+    int fname(env_t *e, int *hdr, int *sup_off, int *sup, double *c2d, int *load_off, int *load_upper, int *load_alias, double *load4, \
+              int *poly_off, double *poly2, double *own4, int cap_e, int cap_p) {                                                      \
+        int ns = 0, nl = 0, np_ = 0, tail = 0;                                                                                         \
+        const Box *fb = e->n_boxes < max_boxes ? &e->boxes[e->n_boxes] : NULL;                                                         \
+        for (int u = 0; u < e->n_boxes; u++) {                                                                                         \
+            const Box *b = &e->boxes[u];                                                                                               \
+            sup_off[u] = ns; load_off[u] = nl; poly_off[u] = np_;                                                                      \
+            if (ns + b->n_be > cap_e || nl + b->n_up > cap_e || np_ + b->n_poly > cap_p) return -1;                                    \
+            for (int i = 0; i < b->n_be; i++, ns++) { sup[ns] = b->be_box[i]; c2d[2 * ns] = b->be_c2d[i][0]; c2d[2 * ns + 1] = b->be_c2d[i][1]; } \
+            for (int i = 0; i < b->n_up; i++, nl++) {                                                                                  \
+                const Box *ub = NULL;                                                                                                  \
+                int idx = -1;                                                                                                          \
+                for (int t = 0; t < e->n_boxes; t++)                                                                                   \
+                    if (e->boxes[t].serial == b->up[i].key) { idx = t; ub = &e->boxes[t]; }                                            \
+                if (idx < 0 && fb && fb->serial == b->up[i].key) { idx = e->n_boxes; tail = 1; }                                       \
+                if (idx < 0) return -1;                                                                                                \
+                const Stack *s = (e->alias_mode && b->up[i].alias && ub) ? &ub->thisStack : &b->up[i].s;                               \
+                load_upper[nl] = idx; load_alias[nl] = b->up[i].alias;                                                                 \
+                load4[4 * nl] = s->c[0]; load4[4 * nl + 1] = s->c[1]; load4[4 * nl + 2] = s->c[2]; load4[4 * nl + 3] = s->m;           \
+            }                                                                                                                          \
+            for (int i = 0; i < b->n_poly; i++, np_++) { poly2[2 * np_] = b->poly[i][0]; poly2[2 * np_ + 1] = b->poly[i][1]; }         \
+            own4[4 * u] = b->thisStack.c[0]; own4[4 * u + 1] = b->thisStack.c[1]; own4[4 * u + 2] = b->thisStack.c[2]; own4[4 * u + 3] = b->thisStack.m; \
+        }                                                                                                                              \
+        sup_off[e->n_boxes] = ns; load_off[e->n_boxes] = nl; poly_off[e->n_boxes] = np_;                                               \
+        hdr[0] = e->n_boxes; hdr[1] = nl; hdr[2] = tail; hdr[3] = tail ? fb->n_be : 0; hdr[4] = tail ? fb->n_poly : 0; hdr[5] = e->alias_mode; \
+        return 0;                                                                                                                      \
+    }
+
 #endif

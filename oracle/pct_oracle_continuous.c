@@ -590,6 +590,7 @@ int pctc_get_candidates(pctc_env *e, double *out6, int *feas, int cap) {
 int pctc_get_packed(pctc_env *e, double *out7, int cap) { int n = e->n_packed < cap ? e->n_packed : cap; memcpy(out7, e->packed, sizeof(double[7]) * n); return e->n_packed; }
 int pctc_n_lstsq(pctc_env *e) { return e->n_lstsq; }
 int pctc_n_ems_intermediate(pctc_env *e) { return e->last_ntmp; }
+PO_DEFINE_GET_SUPPORT_GRAPH(pctc_get_support_graph, pctc_env, PC_MAX_BOXES)
 
 /* What heuristic.py reads from a PackingContinuous env (heuristic.py:163-166,190-193,387-416,541-567):
  * Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) (C:space.py:380-425; max_h is

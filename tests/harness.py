@@ -219,3 +219,101 @@ def sequential_eval(make_env, episodes, nb=80, nl=50):
                 out.append((float(info["ratio"]), int(info["counter"]), [list(p) for p in items]))
                 break
     return out
+
+
+# ---- the support graph an env keeps between steps (stability settings) -----------------------------------------------------
+POLY_MAX = 256  # csrc/pct_kernels.h: entries of an env's polygon pool
+
+
+def _bits(a):
+    return np.ascontiguousarray(a, dtype=np.float64).view(np.uint64)
+
+
+def _fma(a, b, c):
+    """a * b + c rounded once (math.fma arrives with Python 3.13)"""
+    from fractions import Fraction
+    return float(Fraction(a) * Fraction(b) + Fraction(c))
+
+
+def split_direction(c2d):
+    """the two-support split direction from the two contact centres (D:space.py:107-112: the line through them over its squared length;
+    np.linalg.norm of a 2-vector = sqrt of the ddot, whose second product is fused)"""
+    import math
+    lx, ly = float(c2d[0][0] - c2d[1][0]), float(c2d[0][1] - c2d[1][1])
+    ln = math.sqrt(_fma(ly, ly, lx * lx))
+    return np.array([lx / (ln * ln), ly / (ln * ln)])
+
+
+def compare_graphs(dev, orc, where=""):
+    """Compare two support graphs in the CANONICAL FORM: per env, slot-independent,
+
+        per placed box u, in placement order:
+          supports[u]   indices of the boxes u rests on, in stored order (= scan order at its placement, the reference's bottom_edges)
+          loads[u]      rows (cx, cy, cz, mass) resting on u in insertion order (the reference's up_edges dict), with load_upper[u] = the box each
+                        comes from and load_alias[u] = the entry is that box's own stack object
+          polygon[u]    stored shrunk support polygon, vertices in stored order (empty if none is stored)
+          own_stack[u]  (cx, cy, cz, mass) of the box's own stack (alias mode only)
+        counts n_box, n_edge, n_poly
+
+    `dev` is the product's side (PctBatch.support_graph / the host build's decoder), `orc` the oracle's (Oracle*.support_graph).  Floats are
+    compared as bit patterns, never with a tolerance.  What each side holds, and what is therefore compared how:
+      * cz of a load: virtual walks do not carry it, real placements store it on both sides -> compared like the other columns.
+      * a load's value is the one the next walk reads: in alias mode the oracle reads an object entry through the upper box's live stack;
+        the device keeps that value in the stored load too (after a completed descent they are equal, after a failed one alias_sync_loads
+        copies them) -> compared, and the device's object entries must equal the upper box's own_stack.
+      * box index n_box = the box of a FAILED real placement.  Both sides keep the entries its descent wrote until the env resets (the
+        reference's up_edges keep them under a key no live box has, so they keep their last value; the device keeps the pool's tail).
+      * polygons: the device stores one only for boxes with >= 2 supports (a single support is a rectangle test in registers, pinned by
+        tests/test_gpu_geometry_units.py) and only while the pool has room (else the walk recomputes it) -> single-support polygons of the
+        oracle are not compared; with >= 2 supports the device's is the oracle's, or empty exactly when it did not fit.
+      * n_poly counts pool entries: vertices of the stored polygons plus one split direction per stored two-support box, the failed box's included.
+      * the split direction has no oracle field -> compared with split_direction() of the oracle's two contact centres.
+      * own_stack of a box that rests on the floor and carries nothing is never written by the device and never read -> not compared.
+      * alias bits at or beyond n_edge are leftovers of earlier episodes (every appended edge rewrites its bit) -> reported, not compared.
+    Raises AssertionError naming box and field; returns the numbers of compared loads / vertices / splits / own stacks."""
+    n = dict(loads=0, vertices=0, splits=0, own=0)
+    assert dev["n_box"] == orc["n_box"], "%s n_box: %d, oracle %d" % (where, dev["n_box"], orc["n_box"])
+    assert dev["n_edge"] == orc["n_edge"], "%s n_edge: %d, oracle %d" % (where, dev["n_edge"], orc["n_edge"])
+    both_alias = dev["alias"] and orc["alias"]
+    acc = 0
+    for u in range(dev["n_box"]):
+        w = "%s box %d" % (where, u)
+        assert dev["supports"][u] == orc["supports"][u], "%s supports: %s, oracle %s" % (w, dev["supports"][u], orc["supports"][u])
+        assert dev["load_upper"][u] == orc["load_upper"][u], "%s loads come from boxes %s, oracle %s" % (w, dev["load_upper"][u], orc["load_upper"][u])
+        for i, name in enumerate(("cx", "cy", "cz", "mass")):
+            a, b = _bits(dev["loads"][u][:, i]), _bits(orc["loads"][u][:, i])
+            assert np.array_equal(a, b), "%s load %s: row %d (from box %d) %r, oracle %r" % (
+                w, name, int(np.nonzero(a != b)[0][0]), dev["load_upper"][u][int(np.nonzero(a != b)[0][0])],
+                dev["loads"][u][int(np.nonzero(a != b)[0][0]), i], orc["loads"][u][int(np.nonzero(a != b)[0][0]), i])
+        n["loads"] += len(dev["load_upper"][u])
+        if both_alias:
+            assert dev["load_alias"][u] == orc["load_alias"][u], "%s load is_alias: %s, oracle %s" % (w, dev["load_alias"][u], orc["load_alias"][u])
+        if dev["alias"]:
+            for i, (up, al) in enumerate(zip(dev["load_upper"][u], dev["load_alias"][u])):
+                if al and up < dev["n_box"]:
+                    assert np.array_equal(_bits(dev["loads"][u][i]), _bits(dev["own_stack"][up])), \
+                        "%s load row %d is box %d's own stack object but holds %s, own_stack %s" % (w, i, up, dev["loads"][u][i], dev["own_stack"][up])
+        k, m = len(orc["supports"][u]), len(orc["polygon"][u])
+        stored = k >= 2 and acc + m + (k == 2) <= POLY_MAX
+        if stored:
+            assert dev["poly_pos"][u] == acc, "%s polygon pool position %d, expected %d" % (w, dev["poly_pos"][u], acc)
+            assert dev["polygon"][u].shape == orc["polygon"][u].shape and np.array_equal(_bits(dev["polygon"][u]), _bits(orc["polygon"][u])), \
+                "%s polygon: %s, oracle %s" % (w, dev["polygon"][u].tolist(), orc["polygon"][u].tolist())
+            n["vertices"] += m
+            acc += m + (k == 2)
+            if k == 2:
+                want = split_direction(orc["c2d"][u])
+                assert dev["split"][u] is not None and np.array_equal(_bits(dev["split"][u]), _bits(want)), \
+                    "%s split direction: %s, from the contact centres %s" % (w, dev["split"][u], want)
+                n["splits"] += 1
+        else:
+            assert len(dev["polygon"][u]) == 0, "%s polygon: %d vertices stored where none is expected (%d supports)" % (w, len(dev["polygon"][u]), k)
+        if both_alias and (k >= 1 or len(orc["load_upper"][u])):
+            assert np.array_equal(_bits(dev["own_stack"][u]), _bits(orc["own_stack"][u])), \
+                "%s own_stack: %s, oracle %s" % (w, dev["own_stack"][u], orc["own_stack"][u])
+            n["own"] += 1
+    has, k, m = orc["failed_box"]
+    if has and k >= 2 and acc + m + (k == 2) <= POLY_MAX:
+        acc += m + (k == 2)
+    assert dev["n_poly"] == acc, "%s n_poly: %d, expected %d" % (where, dev["n_poly"], acc)
+    return n

@@ -35,6 +35,7 @@ static int g_use_v2 = 0;  // sh_use_v2: route the virtual checks through stab_vi
 #include "pct_pyhash.cuh"
 #include "pct_geom.cuh"
 #include "pct_geom_continuous.cuh"
+#include "pct_support_graph.h"
 
 using namespace pct;
 
@@ -150,7 +151,7 @@ int sh_place(StabHost *h, int x, int y, int z, int lx, int ly, double density) {
     const int n0 = h->n_box;  // may equal the holder size: the kernel (like the reference) runs the check first and rejects the box afterwards
     h->e_off[n0] = (uint16_t)h->n_edge;
     h->poly_off[n0] = (uint16_t)h->n_poly;
-    h->first_in[n0 < NB_MAX ? n0 : 0] = EDGE_NIL;
+    if (n0 < NB_MAX) h->first_in[n0] = EDGE_NIL;
     const int mh = rest_height(h->box, 0, n0, 1, lx, ly, lx + x, ly + y);
     if (lx + x > h->W || ly + y > h->L) return 0;
     if (mh + z > h->H) return 0;
@@ -280,7 +281,7 @@ int shc_place_row(StabHostC *h, const double a[6], const double nb[3], double de
     lx = around6(lx); ly = around6(ly);
     const int n0 = h->n_box;
     bool ok = !(lx + x - 1e-6 > h->W || ly + y - 1e-6 > h->L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
-    h->e_off[n0] = (uint16_t)h->n_edge; h->poly_off[n0] = (uint16_t)h->n_poly; h->first_in[n0 < NB_MAX ? n0 : 0] = EDGE_NIL;
+    h->e_off[n0] = (uint16_t)h->n_edge; h->poly_off[n0] = (uint16_t)h->n_poly; if (n0 < NB_MAX) h->first_in[n0] = EDGE_NIL;
     if (!ok) return 0;
     double mh = rest_height_c(h->box, 0, n0, 1, lx, ly, lx + x, ly + y);
     const double max_h = mh < 0 ? 0.0 : mh;
@@ -308,11 +309,19 @@ int shc_place_row(StabHostC *h, const double a[6], const double nb[3], double de
 }
 }
 
-// debug / triage: the incoming loads of placed box i in pool order -> rows (edge position, cx, cy, cz, m); returns their number
-extern "C" int sh_incoming(StabHost *h, int i, double *out5, int cap) {
-    int n = 0;
-    for (int q = h->first_in[i]; q != EDGE_NIL && n < cap; q = h->e_next[q], n++) {
-        out5[5 * n] = q; out5[5 * n + 1] = h->e_st[q].cx; out5[5 * n + 2] = h->e_st[q].cy; out5[5 * n + 3] = h->e_st[q].cz; out5[5 * n + 4] = h->e_st[q].m;
-    }
-    return n;
+// The support graph the pools hold, through the decoder the C ABI runs on the device records (csrc/pct_support_graph.h): 1 = decoded, 0 = finding in err.
+// sh_pool_field: address of one pool array (0 e_st, 1 e_next, 2 e_alias), so a test can damage a record and see the decoder / the comparison name it.
+template <class H>
+static int graph_of(H *h, pct_support_graph *out, char *err, int cap) {
+    const GraphRecord r{h->n_box, h->n_edge, h->n_poly, h->e_off, h->poly_off, h->e_lower, h->e_next, h->first_in, h->last_in, h->e_st, &h->poly[0][0],
+                        h->alias ? h->box_st : nullptr, h->alias ? h->e_upper : nullptr, h->alias ? h->e_alias : nullptr};
+    return decode_support_graph(r, out, err, (size_t)cap) ? 1 : 0;
+}
+template <class H>
+static void *field_of(H *h, int which) { return which == 0 ? (void *)h->e_st : which == 1 ? (void *)h->e_next : (void *)h->e_alias; }
+extern "C" {
+int sh_support_graph(StabHost *h, pct_support_graph *out, char *err, int cap) { return graph_of(h, out, err, cap); }
+int shc_support_graph(StabHostC *h, pct_support_graph *out, char *err, int cap) { return graph_of(h, out, err, cap); }
+void *sh_pool_field(StabHost *h, int which) { return field_of(h, which); }
+void *shc_pool_field(StabHostC *h, int which) { return field_of(h, which); }
 }

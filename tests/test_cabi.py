@@ -33,6 +33,7 @@ def test_struct_layouts_match_header():
     m = import_module("pct_b200._lib")
     assert C.sizeof(m.StepInfo) == 32
     assert C.sizeof(m.StateDump) == 16 + 8 + 24 + 8 + 80 * 7 * 8 + 256 * 6 * 8
+    assert C.sizeof(m.SupportGraph) == 4 * (6 + 5 * 82 + 3 * 256) + 8 * (256 * 4 + 256 * 2 + 82 * 2 + 82 * 4) == 20960
     assert C.sizeof(m.Config) == 112  # + shuffle (round 2); pct_api.cu static_asserts the C side
 
 

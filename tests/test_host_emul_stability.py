@@ -31,7 +31,7 @@ def lib():
     inc = _cuda_include()
     if inc is None:
         pytest.skip("CUDA headers not found")
-    deps = [SRC] + [os.path.join(CSRC, f) for f in ("pct_stability.cuh", "pct_geom.cuh", "pct_geom_continuous.cuh", "pct_kernels.h", "pct_pyhash.cuh")]
+    deps = [SRC] + [os.path.join(CSRC, f) for f in ("pct_stability.cuh", "pct_geom.cuh", "pct_geom_continuous.cuh", "pct_kernels.h", "pct_pyhash.cuh", "pct_support_graph.h")]
     if not os.path.exists(OUT) or any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in deps):
         os.makedirs(os.path.dirname(OUT), exist_ok=True)
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I" + CSRC,
@@ -55,6 +55,11 @@ def lib():
     L.shc_set_alias.argtypes = [C.c_void_p, C.c_int]
     L.shc_virtual.argtypes = [C.c_void_p, dp, C.c_double]
     L.shc_place_row.argtypes = [C.c_void_p, dp, dp, C.c_double]
+    for f in ("sh_support_graph", "shc_support_graph"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int]
+    for f in ("sh_pool_field", "shc_pool_field"):
+        getattr(L, f).restype = C.c_void_p
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int]
     return L
 
 
