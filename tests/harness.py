@@ -67,6 +67,24 @@ NEEDS_ALIAS = ("alias_s1",)  # records only the object-alias semantics (the defa
 #                              snapshot mode (PCT_ORACLE_ALIAS=0 / PCT_B200_ALIAS=0) must NOT: tests/test_oracle_golden.py
 
 
+# continuous: containers other than the unit cube, each in settings 1-3 (tests/golden/make_cbin_golden.py records them from the reference,
+# tests/test_gpu_continuous_bins.py drives them on the GPU).  Item bounds as tools.py:178-181 computes them: 0.1 / 0.5 x min side.
+#   pallet  non-dyadic sides, W != L != H: the 1e-6 tolerances and the 6-decimal rounding act on sums that are not exact in binary
+#   ten     the reference constructor's default container (C:bin3D.py:11)
+#   mm      a bin in millimetres with sides past 2200, where around6 leaves its fast path for the exact division
+CBIN_CONTAINERS = {"pallet": (1.2, 0.8, 1.0), "ten": (10.0, 10.0, 10.0), "mm": (2400.0, 1700.0, 2300.0)}
+CONT_BINS = {"%s_s%d" % (b, s): dict(_ccase(s, c, 0.1 * min(c), 0.5 * min(c), steps=70), bin=b)
+             for b, c in CBIN_CONTAINERS.items() for s in (1, 2, 3)}
+CONT_BINS["pallet_s1"]["hseed"] = 9194  # heuristic stream whose episodes place boxes flush with x = W (the default seed's only reach y = L)
+
+
+def cont_item_set(c):
+    """the 125 sizes of CONT_ITEM_SET times the container's min side: BR counts the sizes that fit an EMS.  Unrounded, so that its
+    smallest entry is 0.1 * min side = c['low'], the size_minimum the reference derives from an item set (C:bin3D.py:29)"""
+    m = min(c["container"])
+    return [tuple(v * m for v in it) for it in CONT_ITEM_SET]
+
+
 def cont_case_stream(c, seed, env, n):
     """x, y = round(U(lo, hi), 3); z likewise (setting 2) or one of five levels (C:bin3D.py:103-115 scaled to the container)"""
     s = np.zeros((n, 4))
