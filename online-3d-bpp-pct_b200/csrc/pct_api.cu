@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "pct_kernels.h"
+#include "pct_continuous.cuh"
 #include "pct_handle.h"
 #include "pct_support_graph.h"
 
@@ -26,30 +27,9 @@ static_assert(sizeof(pct_config) == 112 && sizeof(pct_step_info) == 32 && sizeof
     } while (0)
 
 namespace pct {
-// continuous domain (pct_continuous.cu)
-int continuous_create(pct_env_batch *h);
-void continuous_destroy(pct_env_batch *h);
-int continuous_launch(pct_env_batch *h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
-                      uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre = nullptr);
-int continuous_preview(pct_env_batch *h, const ItemParams &ip, cudaStream_t st);
-int continuous_policy_random(pct_env_batch *h, int32_t *leaf_idx, uint64_t seed, int64_t t, cudaStream_t st);
-int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out);
-int continuous_get_support_graph(pct_env_batch *h, int env, const DEnvAux *aux, pct_support_graph *out, char *err, size_t cap);
-int64_t continuous_state_bytes();
-int continuous_heuristic(pct_env_batch *h, int code, double *rows, double *hstate, cudaStream_t st);
-int continuous_query(pct_env_batch *h, int env, const double q[5], double density, double *d_out, cudaStream_t st);
-int continuous_queries(pct_env_batch *h, const QParams &q, cudaStream_t st);
-// snapshot / restore (pct_snapshot.cu)
-int64_t snapshot_record_bytes(const pct_env_batch *h);
-uint64_t snapshot_fingerprint(const pct_env_batch *h);
-cudaError_t launch_snapshot(pct_env_batch *h, const int32_t *env, int n, void *buf, cudaStream_t st);
-cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, void *obs, cudaStream_t st);
-}  // namespace pct
-
-namespace pct {
-// the step's pools of stability walks: worst-case capacity, only the used prefix is ever touched.  Continuation pool: WalkCont entries for the
-// sequential kernel, the (larger) piece queue + its flags and per-walk counters only with PCT_B200_WALK=fork
-cudaError_t create_walk_pools(pct_env_batch *h, size_t item_bytes) {
+// the step's pools of stability walks, with queue entries of `item_bytes` (WalkItem / WalkItemC): worst-case capacity, only the used prefix is ever
+// touched.  Continuation pool: WalkCont entries for the sequential kernel, the (larger) piece queue + its flags and per-walk counters only with PCT_B200_WALK=fork
+static cudaError_t create_walk_pools(pct_env_batch *h, size_t item_bytes) {
     const size_t n = (size_t)h->n_envs;
     h->contq_env_bytes = h->walk_fork ? sizeof(WalkPiece) * (size_t)WALK_PIECES_PER_ENV : sizeof(WalkCont) * (size_t)WALK_CONT_PER_ENV;
     cudaError_t e = cudaMalloc(&h->d_walkq, item_bytes * (size_t)CAND_MAX * n);
@@ -74,6 +54,46 @@ cudaError_t sm_count(int *n) {
     return e;
 }
 }  // namespace pct
+
+// The kernel parameters that come from the config, the item source and the env range [off, off + cnt), for every kernel of the domain; each
+// call sets its own fields on top (buffers, mode, hand-over flags, delta / alias state, walk pools, order).
+static DParams discrete_params(const pct_env_batch *h, int off, int cnt) {
+    DParams p{};
+    p.hot = h->d_hot + off; p.cold = h->d_cold + off; p.n_envs = cnt;
+    p.W = (int)h->cfg.container_size[0]; p.L = (int)h->cfg.container_size[1]; p.H = (int)h->cfg.container_size[2];
+    p.nb = h->cfg.internal_node_holder; p.nl = h->cfg.leaf_node_holder; p.setting = h->cfg.setting;
+    p.low_bound = h->cfg.size_minimum; p.lnes = h->cfg.lnes; p.shuffle = h->cfg.shuffle;
+    p.item_mode = h->item_mode; p.item_set = h->d_item_set; p.n_items = h->n_items;
+    p.stream = h->d_stream ? h->d_stream + (size_t)off * h->stream_len * 4 : nullptr; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
+    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base + off; p.env_id_base0 = h->cfg.env_id_base;
+    p.obs_f64 = h->cfg.obs_dtype == PCT_F64; p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
+    return p;
+}
+static CParams continuous_params(const pct_env_batch *h) {
+    CParams p{};
+    p.env = h->d_cenv; p.n_envs = h->n_envs;
+    p.W = h->cfg.container_size[0]; p.L = h->cfg.container_size[1]; p.H = h->cfg.container_size[2];
+    p.nb = h->cfg.internal_node_holder; p.nl = h->cfg.leaf_node_holder; p.setting = h->cfg.setting;
+    p.low_bound = h->cfg.size_minimum; p.shuffle = h->cfg.shuffle;
+    p.item_mode = h->item_mode; p.sample_dist = h->cfg.sample_from_distribution;
+    p.sample_a = h->cfg.sample_left_bound; p.sample_b = h->cfg.sample_right_bound;
+    p.item_set = h->d_item_set; p.n_items = h->n_items; p.stream = h->d_stream; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
+    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base;
+    p.obs_f64 = h->cfg.obs_dtype == PCT_F64; p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
+    return p;
+}
+
+// env range gi of the batch cut into G contiguous ranges
+static void env_range(const pct_env_batch *h, int gi, int G, int &off, int &cnt) {
+    off = (int)((int64_t)h->n_envs * gi / G);
+    cnt = (int)((int64_t)h->n_envs * (gi + 1) / G) - off;
+}
+
+static bool capturing(cudaStream_t st) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(st, &cap);
+    return cap != cudaStreamCaptureStatusNone;
+}
 
 extern "C" {
 
@@ -169,36 +189,35 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
         if (e == cudaSuccess) e = cudaMemset(h->d_hstate_c, 0, sizeof(double) * 4 * (size_t)n_envs);
     }
     h->snap_fp = snapshot_fingerprint(h);
-    if (e == cudaSuccess) {
-        if (cfg->domain == PCT_DISCRETE) {
-            e = cudaMalloc(&h->d_hot, sizeof(DEnvHot) * (size_t)n_envs);
-            if (e == cudaSuccess) e = cudaMalloc(&h->d_cold, sizeof(DEnvCold) * (size_t)n_envs);
-            if (e == cudaSuccess) e = cudaMemset(h->d_hot, 0, sizeof(DEnvHot) * (size_t)n_envs);
-            if (e == cudaSuccess) e = cudaMalloc(&h->d_ready, sizeof(int32_t) * 2 * (size_t)n_envs);
-            if (e == cudaSuccess) e = cudaMemset(h->d_ready, 0, sizeof(int32_t) * 2 * (size_t)n_envs);
-            if (e == cudaSuccess) e = cudaMemset(h->d_cold, 0, sizeof(DEnvCold) * (size_t)n_envs);
-            // HM / MACS / RANDOM on a bin wider than 32 cells run with dynamic shared memory: raise its limit here, so that
-            // pct_heuristic_actions stays enqueue-only (capturable)
-            if (e == cudaSuccess && (cfg->container_size[0] > HEUR_SIDE_MAX || cfg->container_size[1] > HEUR_SIDE_MAX)) e = prepare_heuristic_big();
-            if (e == cudaSuccess && !h->k3_block) e = create_walk_pools(h, sizeof(WalkItem));
-            h->lpt = !h->k3_block;   // heaviest-env-first block order (pct_discrete.cu, order_lookup / order_file); PCT_B200_LPT=0 disables
-            if (const char *lv = getenv("PCT_B200_LPT")) h->lpt = atoi(lv) != 0 && !h->k3_block;
-            if (e == cudaSuccess && h->lpt) {
-                // parity + two 64-bucket histograms + two sets of per-bucket env lists; starts as "every env in the lightest bucket, in env order"
-                const size_t words = 2 + 2 * 64 + 2 * 64 * (size_t)n_envs;
-                e = cudaMalloc(&h->d_order, sizeof(int32_t) * words);
-                if (e == cudaSuccess) e = cudaMemset(h->d_order, 0, sizeof(int32_t) * words);
-                if (e == cudaSuccess) {
-                    std::vector<int32_t> id((size_t)n_envs);
-                    for (int i = 0; i < n_envs; i++) id[i] = i;
-                    const int32_t n32 = n_envs;
-                    e = cudaMemcpy(h->d_order + 2 + 63, &n32, sizeof n32, cudaMemcpyHostToDevice);
-                    if (e == cudaSuccess) e = cudaMemcpy(h->d_order + 2 + 128 + 63 * (size_t)n_envs, id.data(), sizeof(int32_t) * id.size(), cudaMemcpyHostToDevice);
-                }
-            }
-        } else {
-            int rc = continuous_create(h);
-            if (rc != PCT_OK) { g_create_err = h->err; delete h; return rc; }
+    const bool disc = cfg->domain == PCT_DISCRETE;
+    if (e == cudaSuccess) e = cudaMalloc(&h->d_ready, sizeof(int32_t) * 2 * (size_t)n_envs);
+    if (e == cudaSuccess) e = cudaMemset(h->d_ready, 0, sizeof(int32_t) * 2 * (size_t)n_envs);
+    if (disc) {
+        if (e == cudaSuccess) e = cudaMalloc(&h->d_hot, sizeof(DEnvHot) * (size_t)n_envs);
+        if (e == cudaSuccess) e = cudaMalloc(&h->d_cold, sizeof(DEnvCold) * (size_t)n_envs);
+        if (e == cudaSuccess) e = cudaMemset(h->d_hot, 0, sizeof(DEnvHot) * (size_t)n_envs);
+        if (e == cudaSuccess) e = cudaMemset(h->d_cold, 0, sizeof(DEnvCold) * (size_t)n_envs);
+        // HM / MACS / RANDOM on a bin wider than 32 cells run with dynamic shared memory: raise its limit here, so that
+        // pct_heuristic_actions stays enqueue-only (capturable)
+        if (e == cudaSuccess && (cfg->container_size[0] > HEUR_SIDE_MAX || cfg->container_size[1] > HEUR_SIDE_MAX)) e = prepare_heuristic_big();
+    } else {
+        if (e == cudaSuccess) e = cudaMalloc(&h->d_cenv, sizeof(CEnv) * (size_t)n_envs);
+        if (e == cudaSuccess) e = cudaMemset(h->d_cenv, 0, sizeof(CEnv) * (size_t)n_envs);
+    }
+    if (e == cudaSuccess && !h->k3_block) e = create_walk_pools(h, disc ? sizeof(WalkItem) : sizeof(WalkItemC));
+    h->lpt = disc && !h->k3_block;   // heaviest-env-first block order (pct_discrete.cu, order_lookup / order_file); PCT_B200_LPT=0 disables
+    if (const char *lv = getenv("PCT_B200_LPT")) h->lpt = h->lpt && atoi(lv) != 0;
+    if (e == cudaSuccess && h->lpt) {
+        // parity + two 64-bucket histograms + two sets of per-bucket env lists; starts as "every env in the lightest bucket, in env order"
+        const size_t words = 2 + 2 * 64 + 2 * 64 * (size_t)n_envs;
+        e = cudaMalloc(&h->d_order, sizeof(int32_t) * words);
+        if (e == cudaSuccess) e = cudaMemset(h->d_order, 0, sizeof(int32_t) * words);
+        if (e == cudaSuccess) {
+            std::vector<int32_t> id((size_t)n_envs);
+            for (int i = 0; i < n_envs; i++) id[i] = i;
+            const int32_t n32 = n_envs;
+            e = cudaMemcpy(h->d_order + 2 + 63, &n32, sizeof n32, cudaMemcpyHostToDevice);
+            if (e == cudaSuccess) e = cudaMemcpy(h->d_order + 2 + 128 + 63 * (size_t)n_envs, id.data(), sizeof(int32_t) * id.size(), cudaMemcpyHostToDevice);
         }
     }
     if (e != cudaSuccess) {
@@ -213,7 +232,7 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
 void pct_destroy(pct_handle h) {
     if (!h) return;
     cudaSetDevice(h->device);
-    if (h->cfg.domain == PCT_CONTINUOUS) continuous_destroy(h);
+    cudaFree(h->d_cenv);
     cudaFree(h->d_order);
     cudaFree(h->d_walkq); cudaFree(h->d_walk_ctr); cudaFree(h->d_contq); cudaFree(h->d_cont_ctr); cudaFree(h->d_piece_ready); cudaFree(h->d_walk_pend);
     cudaFree(h->d_hstate); cudaFree(h->d_hstate_c); cudaFree(h->d_query_c); cudaFree(h->d_query); cudaFree(h->d_aux);
@@ -228,6 +247,9 @@ void pct_destroy(pct_handle h) {
         if (h->ev_join[gi]) cudaEventDestroy(h->ev_join[gi]);
     }
     delete h;
+    // The launchers report cudaGetLastError(), the last error of this thread's runtime (this library's own: it is linked statically). Leave it
+    // clear, so that an error of a handle torn down here (a failed pct_create) is never reported by a later call of another handle.
+    (void)cudaGetLastError();
 }
 
 int pct_set_item_set(pct_handle h, const double *items_xyz, int32_t n_items) {
@@ -273,26 +295,16 @@ static void begin_obs(pct_handle h, const void *obs) {
 static int launch_range(pct_handle h, int mode, int off, int cnt, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs,
                         float *rew, uint8_t *done, pct_step_info *info, cudaStream_t gs, bool whole_batch, const PreKernel *pre = nullptr) {
     const size_t osz = h->cfg.obs_dtype == PCT_F64 ? 8 : 4, asz = action_f64 ? 8 : 4;
-    DParams p{};
-    p.hot = h->d_hot + off; p.cold = h->d_cold + off; p.n_envs = cnt;
-    p.W = (int)h->cfg.container_size[0]; p.L = (int)h->cfg.container_size[1]; p.H = (int)h->cfg.container_size[2];
-    p.nb = h->cfg.internal_node_holder; p.nl = h->cfg.leaf_node_holder; p.setting = h->cfg.setting;
-    p.low_bound = h->cfg.size_minimum; p.lnes = h->cfg.lnes; p.shuffle = h->cfg.shuffle;
-    p.item_mode = h->item_mode; p.item_set = h->d_item_set; p.n_items = h->n_items;
-    p.stream = h->d_stream ? h->d_stream + (size_t)off * h->stream_len * 4 : nullptr; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
-    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base + off; p.env_id_base0 = h->cfg.env_id_base;
+    DParams p = discrete_params(h, off, cnt);
     p.actions = actions ? (const char *)actions + (size_t)off * 9 * asz : nullptr; p.action_f64 = action_f64;
     p.leaf_idx = leaf_idx ? leaf_idx + off : nullptr;
-    p.obs = (char *)obs + (size_t)off * h->obs_len * osz; p.obs_f64 = h->cfg.obs_dtype == PCT_F64;
+    p.obs = (char *)obs + (size_t)off * h->obs_len * osz;
     p.reward = rew ? rew + off : nullptr; p.done = done ? done + off : nullptr; p.info = info ? info + off : nullptr; p.mode = mode;
     p.dbg = (long long *)h->dbg;
     p.order = (h->lpt && whole_batch && !pre) ? h->d_order : nullptr;
-    p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
     // overlapped launch mode: not while a CUDA graph is being captured (the epoch would be frozen into the graph and a replay
     // would find the flags of the previous replay already set), not under the per-kernel profiler, not with the LPT permutation
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(gs, &cap);
-    if (h->overlap && !h->prof_on && cap == cudaStreamCaptureStatusNone && !pre) {
+    if (h->overlap && !h->prof_on && !capturing(gs) && !pre) {
         p.ready = h->d_ready + 2 * (size_t)off;
         p.epoch = ++h->epoch;
     }
@@ -320,6 +332,30 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
     return PCT_OK;
 }
 
+// the continuous step over the whole batch on stream st; pre as in launch_range
+static int launch_continuous_step(pct_handle h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
+                                  uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre = nullptr) {
+    CParams p = continuous_params(h);
+    p.actions = actions; p.action_f64 = action_f64; p.leaf_idx = leaf_idx;
+    p.obs = obs; p.reward = rew; p.done = done; p.info = info; p.mode = mode;
+    // overlapped launch mode (off by default: measured slower in this domain): not while a CUDA graph is being captured (see launch_range);
+    // the emit kernel's programmatic launch neither
+    const bool cap = capturing(st);
+    if (h->overlap_cont && !cap && !pre) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
+    p.aux = h->d_aux;
+    int opt = (h->alias_mode ? PCT_OPT_ALIAS : 0) | (cap ? PCT_OPT_NO_EMIT_PDL : 0) | (h->cont_pre ? PCT_OPT_CONT_PRE : 0);
+    if (h->d_walkq) {
+        p.walk = walk_pools<WalkItemC>(h, 0, p.n_envs);
+        if (h->obs_delta) p.delta = 1;
+        if (h->obs_delta && h->fill_pending) opt |= PCT_OPT_FILL_PREV;
+    }
+    h->fill_pending = false;
+    if (pre) CK(h, pre->items ? launch_set_items_continuous(p, opt, *pre->items, st) : launch_reset_envs_continuous(p, opt, *pre->reset, st));
+    else CK(h, launch_continuous(p, opt, st));
+    h->launches += continuous_kernels_per_step(p);
+    return PCT_OK;
+}
+
 static int check_item_source(pct_handle h) {
     if (h->item_mode == PCT_ITEMS_RANDOM && !(h->cfg.domain == PCT_CONTINUOUS && h->cfg.sample_from_distribution) && !h->d_item_set) {
         h->err = "no item source: call pct_set_item_set or pct_set_item_stream first";
@@ -335,17 +371,14 @@ static int launch(pct_handle h, int mode, const void *actions, int action_f64, c
     if (rc) return rc;
     CK(h, cudaSetDevice(h->device));
     begin_obs(h, obs);
-    if (h->cfg.domain == PCT_CONTINUOUS) {
-        rc = continuous_launch(h, mode, actions, action_f64, leaf_idx, obs, rew, done, info, st);
-        if (rc == PCT_OK) h->launches++;
-        return rc;
-    }
+    if (h->cfg.domain == PCT_CONTINUOUS) return launch_continuous_step(h, mode, actions, action_f64, leaf_idx, obs, rew, done, info, st);
     // PCT_B200_GROUPS > 1: the batch is cut into contiguous env ranges, each enqueued on its own internal stream between a
     // fork and a join event on the caller's stream (measured: no gain for the device-resident path, see DESIGN.md).
     const int G = h->groups;
     if (G > 1) CK(h, cudaEventRecord(h->ev_fork, st));
     for (int gi = 0; gi < G; gi++) {
-        const int off = (int)((int64_t)h->n_envs * gi / G), cnt = (int)((int64_t)h->n_envs * (gi + 1) / G) - off;
+        int off, cnt;
+        env_range(h, gi, G, off, cnt);
         if (cnt <= 0) continue;
         cudaStream_t gs = gi == 0 ? st : h->sub[gi];
         if (gi > 0) CK(h, cudaStreamWaitEvent(gs, h->ev_fork, 0));
@@ -454,7 +487,8 @@ int pct_step_host(pct_handle h, const void *h_actions, int32_t action_f64, const
     const int G = (h->cfg.domain == PCT_DISCRETE && h->n_envs >= 1024) ? h->host_groups : 1;
     if (G > 1) begin_obs(h, h->d_obs);  // G == 1 goes through launch(), which does it
     for (int gi = 0; gi < G; gi++) {
-        const int off = (int)((int64_t)h->n_envs * gi / G), cnt = (int)((int64_t)h->n_envs * (gi + 1) / G) - off;
+        int off, cnt;
+        env_range(h, gi, G, off, cnt);
         if (cnt <= 0) continue;
         cudaStream_t st = gi == 0 ? h->own_stream : h->sub[gi];
         if (h_actions) CK(h, cudaMemcpyAsync((char *)h->d_act + (size_t)off * 9 * asz, (const char *)h_actions + (size_t)off * 9 * asz, (size_t)cnt * 9 * asz, cudaMemcpyHostToDevice, st));
@@ -476,12 +510,9 @@ int pct_policy_random(pct_handle h, int32_t *d_leaf_idx, uint64_t seed, int64_t 
     if (!h || !d_leaf_idx) return PCT_ERR_INVALID;
     if (!h->did_reset) { h->err = "pct_policy_random before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
-    if (h->cfg.domain == PCT_CONTINUOUS) {
-        int rc = continuous_policy_random(h, d_leaf_idx, seed, t, (cudaStream_t)stream);
-        if (rc == PCT_OK) h->launches++;
-        return rc;
-    }
-    CK(h, launch_policy_random_discrete(h->d_hot, h->n_envs, h->cfg.env_id_base, seed, t, d_leaf_idx, (cudaStream_t)stream));
+    if (h->cfg.domain == PCT_CONTINUOUS)
+        CK(h, launch_policy_random_continuous(h->d_cenv, h->n_envs, h->cfg.env_id_base, seed, t, d_leaf_idx, (cudaStream_t)stream));
+    else CK(h, launch_policy_random_discrete(h->d_hot, h->n_envs, h->cfg.env_id_base, seed, t, d_leaf_idx, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -496,29 +527,16 @@ int pct_policy_random_dev(pct_handle h, int32_t *d_leaf_idx, uint64_t seed, cons
     return PCT_OK;
 }
 
-// DParams of the whole batch for the read-only selection kernels (no action / observation buffers)
-static DParams state_params(pct_handle h) {
-    DParams p{};
-    p.hot = h->d_hot; p.cold = h->d_cold; p.n_envs = h->n_envs;
-    p.W = (int)h->cfg.container_size[0]; p.L = (int)h->cfg.container_size[1]; p.H = (int)h->cfg.container_size[2];
-    p.nb = h->cfg.internal_node_holder; p.nl = h->cfg.leaf_node_holder; p.setting = h->cfg.setting;
-    p.low_bound = h->cfg.size_minimum; p.lnes = h->cfg.lnes;
-    p.item_mode = h->item_mode; p.item_set = h->d_item_set; p.n_items = h->n_items;
-    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base; p.env_id_base0 = h->cfg.env_id_base;
-    return p;
-}
-
 int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64_t seed, int64_t t, void *stream) {
     if (!h || !d_rows) return PCT_ERR_INVALID;
     if (heuristic < PCT_H_LSAH || heuristic > PCT_H_RANDOM) { h->err = "pct_heuristic_actions: unknown heuristic"; return PCT_ERR_INVALID; }
     if (h->cfg.domain != PCT_DISCRETE) { h->err = "pct_heuristic_actions: discrete domain only"; return PCT_ERR_INVALID; }
     if (!h->did_reset) { h->err = "pct_heuristic_actions before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
-    DParams p = state_params(h);
     if (heuristic == PCT_H_BR && !h->d_item_set) { h->err = "PCT_H_BR scores an EMS by the item types that fit: call pct_set_item_set"; return PCT_ERR_STATE; }
     HParams hp{};
     hp.code = heuristic; hp.rows = d_rows; hp.hstate = h->d_hstate; hp.seed = seed; hp.t = t;
-    CK(h, launch_heuristic_discrete(p, hp, (cudaStream_t)stream));
+    CK(h, launch_heuristic_discrete(discrete_params(h, 0, h->n_envs), hp, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -533,8 +551,9 @@ int pct_heuristic_actions_f64(pct_handle h, int32_t heuristic, double *d_rows, v
     if (!h->did_reset) { h->err = "pct_heuristic_actions_f64 before pct_reset"; return PCT_ERR_STATE; }
     if (heuristic == PCT_H_BR && !h->d_item_set) { h->err = "PCT_H_BR scores an EMS by the item types that fit: call pct_set_item_set"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
-    int rc = continuous_heuristic(h, heuristic, d_rows, h->d_hstate_c, (cudaStream_t)stream);
-    if (rc != PCT_OK) return rc;
+    HParamsC hp{};
+    hp.code = heuristic; hp.rows = d_rows; hp.hstate = h->d_hstate_c;
+    CK(h, launch_heuristic_continuous(continuous_params(h), hp, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -546,10 +565,11 @@ int pct_query_placement_f64(pct_handle h, int32_t env, const double dims[3], dou
     if (!h->did_reset) { h->err = "pct_query_placement_f64 before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
     if (!h->d_query_c) CK(h, cudaMalloc(&h->d_query_c, sizeof(double) * 2));
-    const double q[5] = {dims[0], dims[1], dims[2], lx, ly};
+    HParamsC hp{};
+    hp.code = PCT_H_QUERY_; hp.q_env = env; hp.q_den = density; hp.q_out = h->d_query_c;
+    hp.q[0] = dims[0]; hp.q[1] = dims[1]; hp.q[2] = dims[2]; hp.q[3] = lx; hp.q[4] = ly;
     CK(h, cudaDeviceSynchronize());
-    int rc = continuous_query(h, env, q, density, h->d_query_c, h->own_stream);
-    if (rc != PCT_OK) return rc;
+    CK(h, launch_heuristic_continuous(continuous_params(h), hp, h->own_stream));
     h->launches++;
     double out[2];
     CK(h, cudaMemcpyAsync(out, h->d_query_c, sizeof out, cudaMemcpyDeviceToHost, h->own_stream));
@@ -565,7 +585,7 @@ int pct_query_placement(pct_handle h, int32_t env, const int32_t dims[3], int32_
     if (h->cfg.domain != PCT_DISCRETE) { h->err = "pct_query_placement: discrete domain only"; return PCT_ERR_INVALID; }
     if (!h->did_reset) { h->err = "pct_query_placement before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
-    DParams p = state_params(h);
+    const DParams p = discrete_params(h, 0, h->n_envs);
     if (p.W > HEUR_SIDE_MAX || p.L > HEUR_SIDE_MAX) { h->err = "pct_query_placement needs container sides <= 32"; return PCT_ERR_INVALID; }
     const size_t cells = (size_t)p.W * p.L;
     if (!h->d_query) CK(h, cudaMalloc(&h->d_query, sizeof(int32_t) * (2 + HEUR_SIDE_MAX * HEUR_SIDE_MAX)));
@@ -605,7 +625,7 @@ int pct_query_placements(pct_handle h, const int32_t *d_env, int32_t n, int32_t 
     if (rc != PCT_OK || n == 0 || k == 0) return rc;
     CK(h, cudaSetDevice(h->device));
     const QParams q{d_env, n, k, d_q, d_density, d_feasible, d_rest_height};
-    CK(h, launch_queries_discrete(state_params(h), q, (cudaStream_t)stream));
+    CK(h, launch_queries_discrete(discrete_params(h, 0, h->n_envs), q, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -617,8 +637,7 @@ int pct_query_placements_f64(pct_handle h, const int32_t *d_env, int32_t n, int3
     if (rc != PCT_OK || n == 0 || k == 0) return rc;
     CK(h, cudaSetDevice(h->device));
     const QParams q{d_env, n, k, d_q, d_density, d_feasible, d_rest_height};
-    rc = continuous_queries(h, q, (cudaStream_t)stream);
-    if (rc != PCT_OK) return rc;
+    CK(h, launch_queries_continuous(continuous_params(h), q, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -631,7 +650,7 @@ int pct_height_maps(pct_handle h, const int32_t *d_env, int32_t n, int32_t *d_ou
     if (n == 0) return PCT_OK;
     if (!d_out) { h->err = "pct_height_maps: d_out is NULL"; return PCT_ERR_INVALID; }
     CK(h, cudaSetDevice(h->device));
-    CK(h, launch_height_maps(state_params(h), d_env, n, d_out, (cudaStream_t)stream));
+    CK(h, launch_height_maps(discrete_params(h, 0, h->n_envs), d_env, n, d_out, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -651,14 +670,8 @@ int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, 
     if (rc != PCT_OK || n == 0) return rc;
     CK(h, cudaSetDevice(h->device));
     const ItemParams ip{d_env, n, k, nullptr, nullptr, d_out};
-    if (h->cfg.domain == PCT_CONTINUOUS) {
-        rc = continuous_preview(h, ip, (cudaStream_t)stream);
-        if (rc != PCT_OK) return rc;
-    } else {
-        DParams p = state_params(h);
-        p.stream = h->d_stream; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
-        CK(h, launch_preview_discrete(p, ip, (cudaStream_t)stream));
-    }
+    if (h->cfg.domain == PCT_CONTINUOUS) CK(h, launch_preview_continuous(continuous_params(h), ip, (cudaStream_t)stream));
+    else CK(h, launch_preview_discrete(discrete_params(h, 0, h->n_envs), ip, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -668,11 +681,7 @@ int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, 
 static int launch_pre(pct_handle h, const PreKernel &pre, void *d_obs, pct_step_info *d_info, cudaStream_t st) {
     CK(h, cudaSetDevice(h->device));
     begin_obs(h, d_obs);
-    if (h->cfg.domain == PCT_CONTINUOUS) {
-        const int rc = continuous_launch(h, 1, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, &pre);
-        if (rc == PCT_OK) h->launches++;
-        return rc;
-    }
+    if (h->cfg.domain == PCT_CONTINUOUS) return launch_continuous_step(h, 1, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, &pre);
     const int rc = launch_range(h, 1, 0, h->n_envs, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, true, &pre);
     h->fill_pending = false;
     return rc;
@@ -704,7 +713,24 @@ int pct_get_state(pct_handle h, int32_t env, pct_state_dump *out) {
     if (!h || !out || env < 0 || env >= h->n_envs) return PCT_ERR_INVALID;
     CK(h, cudaSetDevice(h->device));
     CK(h, cudaDeviceSynchronize());
-    if (h->cfg.domain == PCT_CONTINUOUS) return continuous_get_state(h, env, out);
+    if (h->cfg.domain == PCT_CONTINUOUS) {
+        std::vector<CEnv> ev(1);
+        CK(h, cudaMemcpy(ev.data(), h->d_cenv + env, sizeof(CEnv), cudaMemcpyDeviceToHost));
+        const CEnv &c = ev[0];
+        memset(out, 0, sizeof(*out));
+        out->n_boxes = c.h.n_box; out->n_ems = c.h.n_ems; out->n_leaf = c.h.n_leaf; out->flags = c.h.flags;
+        out->draw_pos = c.h.draw_pos; out->next_den = c.h.next_den;
+        for (int i = 0; i < 3; i++) out->next_box[i] = c.h.next_box[i];
+        for (int i = 0; i < c.h.n_box && i < 80; i++) {
+            const double *b = c.box[i];
+            out->boxes[i][0] = b[0]; out->boxes[i][1] = b[1]; out->boxes[i][2] = b[2];
+            out->boxes[i][3] = b[0] + b[3]; out->boxes[i][4] = b[1] + b[4]; out->boxes[i][5] = b[2] + b[5];
+            out->boxes[i][6] = c.den[i];
+        }
+        for (int i = 0; i < c.h.n_ems && i < 256; i++)
+            for (int t = 0; t < 6; t++) out->ems[i][t] = c.ems[i][t];
+        return PCT_OK;
+    }
     DEnvHot hot;
     std::vector<double> den(NB_MAX);
     CK(h, cudaMemcpy(&hot, h->d_hot + env, sizeof(hot), cudaMemcpyDeviceToHost));
@@ -733,9 +759,13 @@ int pct_get_support_graph(pct_handle h, int32_t env, pct_support_graph *out) {
     char err[256] = "";
     bool ok;
     if (h->cfg.domain == PCT_CONTINUOUS) {
-        const int rc = continuous_get_support_graph(h, env, alias ? aux.data() : nullptr, out, err, sizeof err);
-        if (rc != PCT_OK && rc != PCT_ERR_STATE) { h->err = "pct_get_support_graph: copy of the env record failed"; return rc; }
-        ok = rc == PCT_OK;
+        std::vector<CEnv> ev(1);
+        CK(h, cudaMemcpy(ev.data(), h->d_cenv + env, sizeof(CEnv), cudaMemcpyDeviceToHost));
+        const CEnv &c = ev[0];
+        if (h->cfg.setting == 2) { memset(out, 0, sizeof *out); out->n_box = c.h.n_box; return PCT_OK; }
+        const GraphRecord r{c.h.n_box, c.h.n_edge, c.h.n_poly, c.e_off, c.poly_off, c.e_lower, c.e_next, c.first_in, c.last_in, c.e_st, &c.poly[0][0],
+                            alias ? aux[0].box_st : nullptr, alias ? aux[0].e_upper : nullptr, alias ? aux[0].e_alias : nullptr};
+        ok = decode_support_graph(r, out, err, sizeof err);
     } else {
         std::vector<DEnvHot> hot(1);
         std::vector<Stack4> st(EDGE_MAX + 1);
@@ -772,7 +802,12 @@ int pct_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_
     if (!h->did_reset) { h->err = "pct_restore before pct_reset"; return PCT_ERR_STATE; }
     if (n == 0) return PCT_OK;
     CK(h, cudaSetDevice(h->device));
-    CK(h, launch_restore(h, d_env, d_rec, n, d_buf, d_obs, (cudaStream_t)stream));
+    DParams pd{};
+    CParams pc{};
+    if (h->cfg.domain == PCT_CONTINUOUS) pc = continuous_params(h);
+    else pd = discrete_params(h, 0, h->n_envs);
+    pd.obs = pc.obs = d_obs;
+    CK(h, launch_restore(h, d_env, d_rec, n, d_buf, pd, pc, (cudaStream_t)stream));
     h->launches++;
     return PCT_OK;
 }
@@ -781,8 +816,7 @@ int32_t pct_obs_len(pct_handle h) { return h ? h->obs_len : 0; }
 int32_t pct_num_envs(pct_handle h) { return h ? h->n_envs : 0; }
 int64_t pct_state_bytes_per_env(pct_handle h) {
     if (!h) return 0;
-    if (h->cfg.domain == PCT_CONTINUOUS) return continuous_state_bytes();
-    return (int64_t)(sizeof(DEnvHot) + sizeof(DEnvCold));
+    return h->cfg.domain == PCT_CONTINUOUS ? (int64_t)sizeof(CEnv) : (int64_t)(sizeof(DEnvHot) + sizeof(DEnvCold));
 }
 int64_t pct_kernel_launches(pct_handle h) { return h ? h->launches : 0; }
 int pct_profile_enable(pct_handle h, int32_t on) {

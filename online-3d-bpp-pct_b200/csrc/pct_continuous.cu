@@ -13,11 +13,9 @@
 #include "pct_common.cuh"
 #include "pct_stability.cuh"
 #include "pct_kernels.h"
-#include "pct_handle.h"
 #include "pct_geom_continuous.cuh"
 #include "pct_walks.cuh"
 #include "pct_continuous.cuh"
-#include "pct_support_graph.h"
 
 namespace pct {
 
@@ -918,68 +916,18 @@ __global__ void __launch_bounds__(256) pctc_reset_envs_kernel(const CParams p, c
     }
 }
 
-// ================= host side =================
-int continuous_create(pct_env_batch *h) {
-    cudaError_t e = cudaMalloc(&h->c_state, sizeof(CEnv) * (size_t)h->n_envs);
-    if (e == cudaSuccess) e = cudaMemset(h->c_state, 0, sizeof(CEnv) * (size_t)h->n_envs);
-    if (e == cudaSuccess) e = cudaMalloc(&h->d_ready, sizeof(int32_t) * 2 * (size_t)h->n_envs);
-    if (e == cudaSuccess) e = cudaMemset(h->d_ready, 0, sizeof(int32_t) * 2 * (size_t)h->n_envs);
-    if (e == cudaSuccess && !h->k3_block) e = create_walk_pools(h, sizeof(WalkItemC));
-    if (e != cudaSuccess) { h->err = std::string("continuous_create: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
-    return PCT_OK;
-}
-void continuous_destroy(pct_env_batch *h) { cudaFree(h->c_state); h->c_state = nullptr; }
-int64_t continuous_state_bytes() { return (int64_t)sizeof(CEnv); }
+// ================= launchers (pct_api.cu builds their CParams from the handle) =================
+// number of kernels one reset / step enqueues (for pct_kernel_launches): apply, candidates, [light, walk], emit; round 1's kernels: apply, candidates, feas_emit
+int continuous_kernels_per_step(const CParams &p) { return p.walk.walkq && p.setting != 2 ? 5 : 3; }
 
-// CParams of the whole batch for the kernels that only read the item source (pct_preview_items)
-static CParams item_params(const pct_env_batch *h) {
-    CParams p{};
-    p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs; p.setting = h->cfg.setting;
-    p.item_mode = h->item_mode; p.sample_dist = h->cfg.sample_from_distribution;
-    p.sample_a = h->cfg.sample_left_bound; p.sample_b = h->cfg.sample_right_bound;
-    p.item_set = h->d_item_set; p.n_items = h->n_items; p.stream = h->d_stream; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
-    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base;
-    return p;
-}
-
-int continuous_preview(pct_env_batch *h, const ItemParams &ip, cudaStream_t st) {
-    const int64_t n = (int64_t)ip.n * ip.k;
-    pctc_preview_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(item_params(h), ip);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { h->err = std::string("pct_preview_items: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
-    return PCT_OK;
-}
-
-// pre non-null (pct_set_items / pct_reset_envs): its kernel in place of the apply kernel, then the rest of the step's sequence in plain stream order
-int continuous_launch(pct_env_batch *h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
-                      uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre) {
-    CParams p{};
-    p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs;
-    p.W = h->cfg.container_size[0]; p.L = h->cfg.container_size[1]; p.H = h->cfg.container_size[2];
-    p.low_bound = h->cfg.size_minimum;
-    p.nb = h->cfg.internal_node_holder; p.nl = h->cfg.leaf_node_holder; p.setting = h->cfg.setting;
-    p.item_mode = h->item_mode; p.sample_dist = h->cfg.sample_from_distribution;
-    p.sample_a = h->cfg.sample_left_bound; p.sample_b = h->cfg.sample_right_bound;
-    p.item_set = h->d_item_set; p.n_items = h->n_items; p.stream = h->d_stream; p.stream_len = h->stream_len; p.traj_len = h->traj_len;
-    p.seed = h->cfg.seed; p.env_id_base = h->cfg.env_id_base; p.shuffle = h->cfg.shuffle;
-    p.actions = actions; p.action_f64 = action_f64; p.leaf_idx = leaf_idx;
-    p.obs = obs; p.obs_f64 = h->cfg.obs_dtype == PCT_F64; p.reward = rew; p.done = done; p.info = info;
-    p.mode = mode; p.keep_draw = h->did_reset ? 1 : 0; p.no_auto_reset = h->cfg.no_auto_reset;
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cap);
-    if (h->overlap_cont && h->d_ready && cap == cudaStreamCaptureStatusNone && !pre) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
+cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply) {
     const bool stab = p.setting != 2;
     const int b2 = (p.n_envs + 1) / 2;
-    if (pre && pre->items) {
-        const int n = max(pre->items->n, p.n_envs);
-        pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, *pre->items);
-    } else if (pre) {
-        pctc_reset_envs_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, *pre->reset);
-    } else if (stab && h->alias_mode && h->d_aux) {
-        p.aux = h->d_aux;
-        pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);
-    } else if (stab) pctc_apply_kernel<true><<<b2, 64, 0, st>>>(p);
-    else pctc_apply_kernel<false><<<b2, 64, 0, st>>>(p);
+    if (apply) {
+        if (stab && (opt & PCT_OPT_ALIAS)) pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);
+        else if (stab) pctc_apply_kernel<true><<<b2, 64, 0, st>>>(p);
+        else pctc_apply_kernel<false><<<b2, 64, 0, st>>>(p);
+    }
     // candidates / feas_emit: with p.ready as programmatic dependent launches (their blocks become resident during the previous
     // kernel's tail and wait per env on the hand-over flags), else plain back-to-back launches
     cudaLaunchAttribute at[1];
@@ -987,90 +935,62 @@ int continuous_launch(pct_env_batch *h, int mode, const void *actions, int actio
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t cfg{};
     cfg.stream = st; cfg.attrs = at; cfg.numAttrs = p.ready ? 1 : 0;
-    const bool pooled = h->d_walkq != nullptr;
-    if (pooled && h->obs_delta && h->d_aux) {  // delta observation rows (emit kernel): a buffer other than the tracked one may hold anything -> "all rows"
-        if (h->fill_pending) launch_fill_prev(h->d_aux, p.n_envs, p.nb, p.nl, st);
-        p.aux = h->d_aux;
-        p.delta = 1;
-    }
-    h->fill_pending = false;
-    if (pooled) p.walk = walk_pools<WalkItemC>(h, 0, p.n_envs);
+    // delta observation rows (emit kernel): a buffer other than the tracked one may hold anything -> "all rows"
+    if (opt & PCT_OPT_FILL_PREV) launch_fill_prev(p.aux, p.n_envs, p.nb, p.nl, st);
     cfg.gridDim = dim3(p.n_envs); cfg.blockDim = dim3(32);
     cudaLaunchKernelEx(&cfg, pctc_candidates_kernel, p);
-    if (pooled) {
+    if (p.walk.walkq) {
         if (stab) {
             int n_sm = 0;
             const cudaError_t es = sm_count(&n_sm);
-            if (es != cudaSuccess) { h->err = std::string("continuous launch: ") + cudaGetErrorString(es); return PCT_ERR_CUDA; }
+            if (es != cudaSuccess) return es;
             pctc_walk_light_kernel<<<n_sm * 4, 32 * LIGHT_WARPS, 0, st>>>(p);
             if (p.walk.walk_fork) pctc_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, 8)), 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
             else pctc_walk_kernel<<<n_sm * 8, 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
         }
-        {
-            cudaLaunchAttribute at2[1];
-            at2[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            at2[0].val.programmaticStreamSerializationAllowed = 1;
-            cudaLaunchConfig_t c2{};
-            c2.stream = st; c2.attrs = at2; c2.numAttrs = (stab && cap == cudaStreamCaptureStatusNone) ? 1 : 0;
-            c2.gridDim = dim3(p.n_envs); c2.blockDim = dim3(64);
-            if (p.obs_f64) cudaLaunchKernelEx(&c2, pctc_emit_kernel<double>, p);
-            else cudaLaunchKernelEx(&c2, pctc_emit_kernel<float>, p);
-        }
-        cudaError_t e2 = cudaGetLastError();
-        if (e2 != cudaSuccess) { h->err = std::string("continuous launch: ") + cudaGetErrorString(e2); return PCT_ERR_CUDA; }
-        h->launches += stab ? 4 : 2;  // apply, candidates, [light, walk], emit; the caller counts one
-        return PCT_OK;
+        cudaLaunchConfig_t c2{};
+        c2.stream = st; c2.attrs = at; c2.numAttrs = (stab && !(opt & PCT_OPT_NO_EMIT_PDL)) ? 1 : 0;
+        c2.gridDim = dim3(p.n_envs); c2.blockDim = dim3(64);
+        if (p.obs_f64) cudaLaunchKernelEx(&c2, pctc_emit_kernel<double>, p);
+        else cudaLaunchKernelEx(&c2, pctc_emit_kernel<float>, p);
+        return cudaGetLastError();
     }
     cfg.blockDim = dim3(64);
-    if (h->cont_pre) {
+    if (opt & PCT_OPT_CONT_PRE) {
         if (p.obs_f64) { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, true, true>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, false, true>, p); }
         else { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, true, true>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, false, true>, p); }
     } else {
         if (p.obs_f64) { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, true, false>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, false, false>, p); }
         else { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, true, false>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, false, false>, p); }
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { h->err = std::string("continuous launch: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
-    h->launches += 2;  // the caller counts one
-    return PCT_OK;
+    return cudaGetLastError();
 }
 
-int continuous_policy_random(pct_env_batch *h, int32_t *leaf_idx, uint64_t seed, int64_t t, cudaStream_t st) {
-    pctc_policy_random_kernel<<<(h->n_envs + 127) / 128, 128, 0, st>>>((const CEnv *)h->c_state, h->n_envs, h->cfg.env_id_base, seed, t, leaf_idx);
-    return cudaGetLastError() == cudaSuccess ? PCT_OK : PCT_ERR_CUDA;
+cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st) {
+    const int n = max(ip.n, p.n_envs);
+    pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, ip);
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    return launch_continuous(p, opt, st, false);
 }
 
-int continuous_get_state(pct_env_batch *h, int env, pct_state_dump *out) {
-    CEnv *tmp = (CEnv *)malloc(sizeof(CEnv));
-    if (cudaMemcpy(tmp, (CEnv *)h->c_state + env, sizeof(CEnv), cudaMemcpyDeviceToHost) != cudaSuccess) { free(tmp); return PCT_ERR_CUDA; }
-    memset(out, 0, sizeof(*out));
-    out->n_boxes = tmp->h.n_box; out->n_ems = tmp->h.n_ems; out->n_leaf = tmp->h.n_leaf; out->flags = tmp->h.flags;
-    out->draw_pos = tmp->h.draw_pos; out->next_den = tmp->h.next_den;
-    for (int i = 0; i < 3; i++) out->next_box[i] = tmp->h.next_box[i];
-    for (int i = 0; i < tmp->h.n_box && i < 80; i++) {
-        const double *b = tmp->box[i];
-        out->boxes[i][0] = b[0]; out->boxes[i][1] = b[1]; out->boxes[i][2] = b[2];
-        out->boxes[i][3] = b[0] + b[3]; out->boxes[i][4] = b[1] + b[4]; out->boxes[i][5] = b[2] + b[5];
-        out->boxes[i][6] = tmp->den[i];
-    }
-    for (int i = 0; i < tmp->h.n_ems && i < 256; i++)
-        for (int t = 0; t < 6; t++) out->ems[i][t] = tmp->ems[i][t];
-    free(tmp);
-    return PCT_OK;
+cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st) {
+    pctc_reset_envs_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, rp);
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    return launch_continuous(p, opt, st, false);
 }
 
-int continuous_get_support_graph(pct_env_batch *h, int env, const DEnvAux *aux, pct_support_graph *out, char *err, size_t cap) {
-    CEnv *tmp = (CEnv *)malloc(sizeof(CEnv));
-    if (cudaMemcpy(tmp, (CEnv *)h->c_state + env, sizeof(CEnv), cudaMemcpyDeviceToHost) != cudaSuccess) { free(tmp); return PCT_ERR_CUDA; }
-    bool ok = true;
-    if (h->cfg.setting == 2) { memset(out, 0, sizeof *out); out->n_box = tmp->h.n_box; }
-    else {
-        const GraphRecord r{tmp->h.n_box, tmp->h.n_edge, tmp->h.n_poly, tmp->e_off, tmp->poly_off, tmp->e_lower, tmp->e_next, tmp->first_in, tmp->last_in,
-                            tmp->e_st, &tmp->poly[0][0], aux ? aux->box_st : nullptr, aux ? aux->e_upper : nullptr, aux ? aux->e_alias : nullptr};
-        ok = decode_support_graph(r, out, err, cap);
-    }
-    free(tmp);
-    return ok ? PCT_OK : PCT_ERR_STATE;
+cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st) {
+    const int64_t n = (int64_t)ip.n * ip.k;
+    pctc_preview_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, ip);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_policy_random_continuous(const CEnv *env, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
+                                            cudaStream_t st) {
+    pctc_policy_random_kernel<<<(n_envs + 127) / 128, 128, 0, st>>>(env, n_envs, env_id_base, seed, t, leaf_idx);
+    return cudaGetLastError();
 }
 
 }  // namespace pct

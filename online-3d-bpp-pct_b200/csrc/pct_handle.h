@@ -14,7 +14,7 @@ struct pct_env_batch {
     // device state
     pct::DEnvHot *d_hot = nullptr;
     pct::DEnvCold *d_cold = nullptr;
-    void *c_state = nullptr;  // continuous-domain state (pct_continuous.cu)
+    pct::CEnv *d_cenv = nullptr;  // continuous-domain state (pct_continuous.cuh)
     double *d_item_set = nullptr;
     int n_items = 0;
     double *d_stream = nullptr;
@@ -78,8 +78,12 @@ struct pct_env_batch {
 };
 
 namespace pct {
-// allocates the pools of the stability walks with queue entries of `item_bytes` (pct_create, continuous_create; not with PCT_B200_K3=block)
-cudaError_t create_walk_pools(pct_env_batch *h, size_t item_bytes);
+// snapshot / restore (pct_snapshot.cu)
+int64_t snapshot_record_bytes(const pct_env_batch *h);
+uint64_t snapshot_fingerprint(const pct_env_batch *h);
+cudaError_t launch_snapshot(pct_env_batch *h, const int32_t *env, int n, void *buf, cudaStream_t st);
+cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, const DParams &pd, const CParams &pc,
+                           cudaStream_t st);
 
 // the pools of the env range [off, off + cnt): env ranges stepped concurrently (pct_step_host's staged path) own disjoint slices
 template <typename Item>

@@ -246,46 +246,18 @@ __global__ void __launch_bounds__(64) pctc_query_kernel(const CParams p, const Q
     }
 }
 
-static CParams state_params_c(pct_env_batch *h) {
-    CParams p{};
-    p.env = (CEnv *)h->c_state; p.n_envs = h->n_envs;
-    p.W = h->cfg.container_size[0]; p.L = h->cfg.container_size[1]; p.H = h->cfg.container_size[2];
-    p.low_bound = h->cfg.size_minimum;
-    p.nb = h->cfg.internal_node_holder; p.nl = h->cfg.leaf_node_holder; p.setting = h->cfg.setting;
-    p.item_set = h->d_item_set; p.n_items = h->n_items;
-    return p;
+// the baselines over the batch, or (hp.code == PCT_H_QUERY_) the single placement query of env hp.q_env
+cudaError_t launch_heuristic_continuous(const CParams &p, const HParamsC &hp, cudaStream_t st) {
+    const int blocks = hp.code == PCT_H_QUERY_ ? 1 : p.n_envs;
+    if (p.setting == 2) pctc_heuristic_kernel<false><<<blocks, 64, 0, st>>>(p, hp);
+    else pctc_heuristic_kernel<true><<<blocks, 64, 0, st>>>(p, hp);
+    return cudaGetLastError();
 }
 
-int continuous_query(pct_env_batch *h, int env, const double q[5], double density, double *d_out, cudaStream_t st) {
-    const CParams p = state_params_c(h);
-    HParamsC hp{};
-    hp.code = PCT_H_QUERY_; hp.q_env = env; hp.q_den = density; hp.q_out = d_out;
-    for (int i = 0; i < 5; i++) hp.q[i] = q[i];
-    if (p.setting == 2) pctc_heuristic_kernel<false><<<1, 64, 0, st>>>(p, hp);
-    else pctc_heuristic_kernel<true><<<1, 64, 0, st>>>(p, hp);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { h->err = std::string("continuous query launch: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
-    return PCT_OK;
-}
-
-int continuous_queries(pct_env_batch *h, const QParams &q, cudaStream_t st) {
-    const CParams p = state_params_c(h);
+cudaError_t launch_queries_continuous(const CParams &p, const QParams &q, cudaStream_t st) {
     if (p.setting == 2) pctc_query_kernel<false><<<q.n, 64, 0, st>>>(p, q);
     else pctc_query_kernel<true><<<q.n, 64, 0, st>>>(p, q);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { h->err = std::string("continuous queries launch: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
-    return PCT_OK;
-}
-
-int continuous_heuristic(pct_env_batch *h, int code, double *rows, double *hstate, cudaStream_t st) {
-    const CParams p = state_params_c(h);
-    HParamsC hp{};
-    hp.code = code; hp.rows = rows; hp.hstate = hstate;
-    if (p.setting == 2) pctc_heuristic_kernel<false><<<p.n_envs, 64, 0, st>>>(p, hp);
-    else pctc_heuristic_kernel<true><<<p.n_envs, 64, 0, st>>>(p, hp);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { h->err = std::string("continuous heuristic launch: ") + cudaGetErrorString(e); return PCT_ERR_CUDA; }
-    return PCT_OK;
+    return cudaGetLastError();
 }
 
 }  // namespace pct

@@ -319,4 +319,22 @@ cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                           cudaStream_t st, const int64_t *t_dev = nullptr);
 
+// ---- continuous domain (pct_continuous.cuh; launchers in pct_continuous.cu, heuristics and queries in pct_heuristics_continuous.cuh) ----
+struct CEnv;
+struct CParams;
+// The host-side choices of a continuous step, passed beside CParams (whose layout is fixed): PCT_OPT_ALIAS (the apply kernel's object semantics
+// of the loads), PCT_OPT_FILL_PREV (reset the delta rows' obs_prev to "all rows" before the candidates kernel), PCT_OPT_NO_EMIT_PDL (emit kernel
+// in plain stream order: while the stream is captured), PCT_OPT_CONT_PRE (round 1's feas_emit kernel: resting heights from pre-rounded rectangles)
+constexpr int PCT_OPT_FILL_PREV = 16, PCT_OPT_CONT_PRE = 32;
+int continuous_kernels_per_step(const CParams &p);
+// apply = false: the sequence without the apply kernel (pct_set_items / pct_reset_envs; p.ready must be nullptr)
+cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply = true);
+cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st);
+cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st);
+cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st);
+cudaError_t launch_queries_continuous(const CParams &p, const QParams &q, cudaStream_t st);
+cudaError_t launch_heuristic_continuous(const CParams &p, const HParamsC &hp, cudaStream_t st);
+cudaError_t launch_policy_random_continuous(const CEnv *env, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
+                                            cudaStream_t st);
+
 }  // namespace pct

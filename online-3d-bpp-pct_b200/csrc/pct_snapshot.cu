@@ -222,7 +222,7 @@ static SnapArgs snap_args(pct_env_batch *h, const int32_t *env, const int32_t *r
     SnapArgs a{};
     a.buf = (unsigned char *)buf; a.env = env; a.rec = rec; a.n = n; a.n_envs = h->n_envs;
     a.stride = snapshot_record_bytes(h); a.fp = h->snap_fp;
-    a.hot = h->d_hot; a.cold = h->d_cold; a.cenv = (CEnv *)h->c_state;
+    a.hot = h->d_hot; a.cold = h->d_cold; a.cenv = h->d_cenv;
     a.aux = h->d_aux; a.alias = h->alias_mode ? 1 : 0;
     a.hstate = h->cfg.domain == PCT_CONTINUOUS ? (void *)h->d_hstate_c : (void *)h->d_hstate;
     a.nb = h->cfg.internal_node_holder; a.nl = h->cfg.leaf_node_holder;
@@ -236,14 +236,10 @@ cudaError_t launch_snapshot(pct_env_batch *h, const int32_t *env, int n, void *b
     return cudaGetLastError();
 }
 
-cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, void *obs, cudaStream_t st) {
+// pd / pc: the parameters of the handle's domain with the observation buffer (nullptr: none); the other struct is not read
+cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, const DParams &pd, const CParams &pc,
+                           cudaStream_t st) {
     const SnapArgs a = snap_args(h, env, rec, n, const_cast<void *>(buf));
-    // the fields the row writers read (write_obs / write_obs_c)
-    DParams pd{};
-    CParams pc{};
-    pd.obs = obs; pd.nb = pc.nb = h->cfg.internal_node_holder; pd.nl = pc.nl = h->cfg.leaf_node_holder;
-    pd.setting = pc.setting = h->cfg.setting; pd.H = (int)h->cfg.container_size[2]; pc.H = h->cfg.container_size[2];
-    pc.obs = obs;
     const bool f64 = h->cfg.obs_dtype == PCT_F64;
     if (h->cfg.domain == PCT_CONTINUOUS) {
         if (f64) pct_restore_kernel<true, double><<<n, SNAP_THREADS, 0, st>>>(a, pd, pc);
