@@ -38,6 +38,23 @@ static __device__ __noinline__ void ddiv3(double a, double b, double c, double d
 static __device__ __noinline__ double dsqrt(double a) { return sqrt(a); }
 __device__ __forceinline__ double dot2(double u0, double u1, double v0, double v1) { return fma(u1, v1, u0 * v0); }
 
+// The rare visits on > KSUP_SMALL supports share the env's one HBM scratch (BigScratch), serialised by a spin lock in global memory.  The walk
+// lanes of one env run in different warps and on different SMs, so both fences are device-scope: the acquire orders the new holder's scratch reads
+// after the lock, the release makes the holder's scratch writes visible before the lock is free.  The host build of this file
+// (tests/host_emul/) runs one walk at a time and needs no fence.
+__device__ __forceinline__ void scratch_lock(int *lock) {
+    while (atomicCAS(lock, 0, 1) != 0) { }
+#ifdef __CUDA_ARCH__
+    __threadfence();
+#endif
+}
+__device__ __forceinline__ void scratch_unlock(int *lock) {
+#ifdef __CUDA_ARCH__
+    __threadfence();
+#endif
+    atomicExch(lock, 0);
+}
+
 __device__ __forceinline__ double slope_of(double ax, double ay, double bx, double by) {
     if (bx != ax) return ddiv(by - ay, bx - ax);
     return (by - ay) * CUDART_INF;  // 0*inf = nan like the reference (convex_hull.py:14)
@@ -542,8 +559,7 @@ static __device__ __noinline__ int stability_check(const G &g, const typename G:
             double (*rect)[4] = S.rect;
             double *px = S.px, *py = S.py, *hx = S.hx, *hy = S.hy;
             if (!small) {  // rare: serialise the lanes of this env on the per-env HBM scratch
-                while (atomicCAS(lock, 0, 1) != 0) { }
-                __threadfence_block();
+                scratch_lock(lock);
                 rect = big->rect; px = big->px; py = big->py; hx = big->hx; hy = big->hy;
             }
 #pragma unroll 1
@@ -645,7 +661,7 @@ static __device__ __noinline__ int stability_check(const G &g, const typename G:
                     }
                 }
             }
-            if (!small) { __threadfence_block(); atomicExch(lock, 0); }
+            if (!small) scratch_unlock(lock);
             SEC(3);
             if (!ok) { SEC_OUT(); return 0; }
             if (depth >= STAB_DEPTH) { flags |= PCT_FLAG_SUPPORT_OVERFLOW; return 0; }
@@ -950,8 +966,7 @@ static __device__ __noinline__ int stab_virtual(const G &g, const typename G::No
                 double (*rect)[4] = lrect;
                 double *px = lpx, *py = lpy, *hx = lhx, *hy = lhy;
                 if (!small) {  // rare: serialise the lanes of this env on the per-env HBM scratch
-                    while (atomicCAS(lock, 0, 1) != 0) { }
-                    __threadfence_block();
+                    scratch_lock(lock);
                     rect = big->rect; px = big->px; py = big->py; hx = big->hx; hy = big->hy;
                 }
 #pragma unroll 1
@@ -1009,7 +1024,7 @@ static __device__ __noinline__ int stab_virtual(const G &g, const typename G::No
                         }
                     }
                 }
-                if (!small) { __threadfence_block(); atomicExch(lock, 0); }
+                if (!small) scratch_unlock(lock);
             }
             if (ok && depth >= STAB_DEPTH) { flags |= PCT_FLAG_SUPPORT_OVERFLOW; ok = false; }
             if (!ok) PCT_STAT(node == NODE_NEW ? 15 : 16);  // heavy visit failed: root / placed box
@@ -1135,8 +1150,7 @@ static __device__ __noinline__ int stab_piece(const G &g, const typename G::Node
         double (*rect)[4] = lrect;
         double *px = lpx, *py = lpy, *hx = lhx, *hy = lhy;
         if (!small) {  // rare: serialise the lanes of this env on the per-env HBM scratch
-            while (atomicCAS(lock, 0, 1) != 0) { }
-            __threadfence_block();
+            scratch_lock(lock);
             rect = big->rect; px = big->px; py = big->py; hx = big->hx; hy = big->hy;
         }
 #pragma unroll 1
@@ -1199,7 +1213,7 @@ static __device__ __noinline__ int stab_piece(const G &g, const typename G::Node
                 fork((int)sup_id[s], (node == NODE_NEW) ? EDGE_NIL : eoff + s, whole ? st.cx : px[s], whole ? st.cy : py[s], sup_m[s]);
             vx = whole ? st.cx : px[0]; vy = whole ? st.cy : py[0]; vm = sup_m[0];
         }
-        if (!small) { __threadfence_block(); atomicExch(lock, 0); }
+        if (!small) scratch_unlock(lock);
         if (!ok) return 0;
         child = sup_id[0];
         skip = (node == NODE_NEW) ? EDGE_NIL : eoff;
