@@ -276,6 +276,28 @@ int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, 
 int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
                   pct_step_info *d_info, void *stream);
 
+/* Leaf expansion of items the envs are not holding, read-only: for a buffer policy (the PCT tree of a buffered state holds the leaves of
+ * each of the B buffered items; choosing a leaf chooses the item) and for lookahead over candidate future items.
+ * Row r expands k items on env d_env[r] (d_env NULL: env r) in its current state:
+ *   d_items  : n x k x 3 sizes, int32 (discrete; clamped to [0, 255] as pct_set_items clamps) / float64 (continuous)
+ *   d_density: n x k densities, or NULL = each env's current item density
+ *   d_leaves : n x k x leaf_node_holder x 9, the handle's observation dtype.  Entry (r, j) holds the leaf rows get_possible_position()
+ *              (D:bin3D.py:100-136, C:bin3D.py) produces for item d_items[r][j]: the first leaf_node_holder feasible candidates in reference
+ *              order as [xs, ys, zs, xe, ye, H, 0, 0, 1], zero rows after the last.  These are the bytes of the leaf rows that pct_set_items
+ *              writes into the observation for that item on that env (same cast, LNES scheme and keyed shuffle, whose keys depend on
+ *              (seed, global env id, draw_pos) only), so leaf l of the expansion is leaf l of pct_set_items(item) and of the step after it.
+ *   d_info   : n x k pct_step_info records, or NULL: the record pct_set_items would write for that env and item: counter, the env's sticky
+ *              flags ORed with the capacity flags this expansion raised, n_leaf, n_cand, n_ems; ratio / ep_reward / ep_len 0.
+ * Read-only: no header field, leaf list, delta-row state or observation row of any env is written, and a flag raised by an expansion goes to
+ * its own record only, so a step after the call behaves exactly as without it.  The call uses the per-env scratch that every step rewrites
+ * before reading it (candidate list, generator and shuffle scratch, the stability test's large-case scratch).  The envs of one call must be
+ * distinct (caller's contract, not checked: that scratch is per env).  An item that fits nowhere (the [100, 100, 100] sentinel) gets zero
+ * leaves; a row whose index is outside [0, n_envs) gets zero rows and zero records.  Enqueue only: no host synchronisation, no allocation
+ * (CUDA-graph capturable).  n == 0: no-op.  Errors: PCT_ERR_STATE before pct_reset; PCT_ERR_INVALID for n < 0, k < 1 or
+ * n * k * leaf_node_holder * 9 > INT32_MAX. */
+int pct_expand_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, const void *d_items, const double *d_density, void *d_leaves,
+                     pct_step_info *d_info, void *stream);
+
 /* env.reset() (D:bin3D.py:61-67, C:bin3D.py:69-75) for chosen envs of the batch: start new episodes in some envs and leave the others
  * as they are.  For gym semantics on a whole batch (no_auto_reset = 1: the caller sees the terminal observation, then resets the
  * finished envs), episode control under auto-reset (time limits, curricula, dropping an episode), and device-resident loops, where a

@@ -394,6 +394,50 @@ class PctBatch(object):
                     "pct_set_items")
         return obs
 
+    def expand_items(self, items, env_idx=None, density=None, out=None):
+        """The leaf rows get_possible_position() (bin3D.py) produces for items the envs are not holding, without changing any env: what a
+        buffer policy chooses from (one leaf of one of the B buffered items) and what lookahead scores.  Enqueued on the current stream
+        (graph-capturable).  items: (n, k, 3) sizes, converted to int32 (discrete) / float64 (continuous); row r expands its k items on env
+        env_idx[r] (default: env r).  density: (n, k) densities (default: each env's current item density).  The envs of one call must be
+        distinct; rows of an index outside [0, n_envs) come out zero.  out: optional preallocated (leaves, info) pair.
+        -> (leaves (n, k, leaf_node_holder, 9) in obs_dtype, info (n, k, 8) int32).  leaves[r, j] are the bytes of the leaf rows
+        set_items(items[r, j]) would write for env env_idx[r], so leaf l here is leaf l of that observation; info[r, j] is the record it
+        would write (decode_info(info.reshape(-1, 8)))."""
+        qd = torch.float64 if self.continuous else torch.int32
+        if not torch.is_tensor(items):
+            items = torch.as_tensor(np.asarray(items))
+        if items.dim() != 3 or items.shape[2] != 3:
+            raise PctError("items must have shape (n, k, 3): [x, y, z] per item")
+        n, k = int(items.shape[0]), int(items.shape[1])
+        if k < 1:
+            raise PctError("expand_items: k must be >= 1")
+        it = items.to(device=self.device, dtype=qd).contiguous()
+        idx = self._index(env_idx, "env_idx")
+        if idx is not None and int(idx.numel()) != n:
+            raise PctError("env_idx must have one entry per item row (%d)" % n)
+        if idx is None and n > self.n_envs:
+            raise PctError("%d item rows without env_idx for %d envs" % (n, self.n_envs))
+        den = None
+        if density is not None:
+            if not torch.is_tensor(density):
+                density = torch.as_tensor(np.asarray(density, dtype=np.float64))
+            if tuple(density.shape) != (n, k):
+                raise PctError("density must have shape (n, k) = (%d, %d)" % (n, k))
+            den = density.to(device=self.device, dtype=torch.float64).contiguous()
+        nl = self.nl
+        if out is None:
+            leaves = torch.empty((n, k, nl, 9), dtype=self.obs_dtype, device=self.device)
+            info = torch.empty((n, k, 8), dtype=torch.int32, device=self.device)
+        else:
+            if len(out) != 2:
+                raise PctError("out must be a (leaves, info) pair")
+            leaves = self._out(out[0], (n, k, nl, 9), self.obs_dtype, "out[0] (leaves)")
+            info = self._out(out[1], (n, k, 8), torch.int32, "out[1] (info)")
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
+        self._check(self.L.pct_expand_items(self.h, ptr(idx), n, k, ptr(it), ptr(den), ptr(leaves), ptr(info), self._stream()),
+                    "pct_expand_items")
+        return leaves, info
+
     # -- host-buffer API (what the reference's VecEnv exchanges over its pipes) --------------------------------
     def reset_host(self, obs_out):
         self._check(self.L.pct_reset_host(self.h, C.c_void_p(obs_out.ctypes.data)), "pct_reset_host")

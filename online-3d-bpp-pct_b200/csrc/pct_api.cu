@@ -676,6 +676,22 @@ int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, 
     return PCT_OK;
 }
 
+int pct_expand_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, const void *d_items, const double *d_density, void *d_leaves,
+                     pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    if (n < 0 || k < 1) { h->err = "pct_expand_items: n must be >= 0 and k >= 1"; return PCT_ERR_INVALID; }
+    if ((int64_t)n * k * h->cfg.leaf_node_holder * 9 > INT32_MAX) { h->err = "pct_expand_items: n * k * leaf_node_holder * 9 overflows int32"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_expand_items before pct_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    if (!d_items || !d_leaves) { h->err = "pct_expand_items: d_items and d_leaves must not be NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    const ExpandParams x{d_env, n, k, d_items, d_density, d_leaves, d_info};
+    if (h->cfg.domain == PCT_CONTINUOUS) CK(h, launch_expand_continuous(continuous_params(h), x, (cudaStream_t)stream));
+    else CK(h, launch_expand_discrete(discrete_params(h, 0, h->n_envs), x, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
 // pct_set_items / pct_reset_envs: the pre-kernel in place of the apply kernel, then the rest of the step's pipeline over the whole batch,
 // on the caller's stream whatever PCT_B200_GROUPS says
 static int launch_pre(pct_handle h, const PreKernel &pre, void *d_obs, pct_step_info *d_info, cudaStream_t st) {

@@ -16,38 +16,12 @@
 #include "pct_geom_continuous.cuh"
 #include "pct_walks.cuh"
 #include "pct_continuous.cuh"
+#include "pct_cand_c.cuh"
 
 namespace pct {
 
 // around6, NodeC / GeomC (geometry policy of the stability routine), rest_height_c, rest_height_pre: pct_geom_continuous.cuh
-
-__device__ __forceinline__ bool rot_dims_c(const double nb[3], int rot, double &sx, double &sy, double &sz) {  // C:space.py:537-559
-    switch (rot) {
-    case 0: sx = nb[0]; sy = nb[1]; sz = nb[2]; return true;
-    case 1: sx = nb[1]; sy = nb[0]; sz = nb[2]; return !(fabs(sx - sy) < 1e-6);
-    case 2: sx = nb[0]; sy = nb[2]; sz = nb[1]; return !(fabs(sx - sy) < 1e-6 && fabs(sy - sz) < 1e-6);
-    case 3: sx = nb[1]; sy = nb[2]; sz = nb[0]; return !(fabs(sx - sy) < 1e-6 && fabs(sy - sz) < 1e-6);
-    case 4: sx = nb[2]; sy = nb[0]; sz = nb[1]; return !(fabs(sx - sy) < 1e-6);
-    default: sx = nb[2]; sy = nb[1]; sz = nb[0]; return !(fabs(sx - sy) < 1e-6);
-    }
-}
-// candidate code = ems_idx << 5 | rot << 2 | corner  ->  the 6-tuple the reference adds to its set (C:space.py:563-566)
-__device__ __forceinline__ void cand_tuple(uint16_t code, const double (*ems)[6], const double nb[3], double t[6]) {
-    const double *m = ems[code >> 5];
-    double sx, sy, sz;
-    rot_dims_c(nb, (code >> 2) & 7, sx, sy, sz);
-    const int q = code & 3;
-    if (q & 1) { t[0] = m[3] - sx; t[3] = m[3]; } else { t[0] = m[0]; t[3] = m[0] + sx; }
-    if (q & 2) { t[1] = m[4] - sy; t[4] = m[4]; } else { t[1] = m[1]; t[4] = m[1] + sy; }
-    t[2] = m[2]; t[5] = m[2] + sz;
-}
-__device__ __noinline__ uint64_t hash_double_call(double v) { return hash_double(v); }  // one copy of the routine for the three call sites of the candidates kernel
-__device__ __noinline__ uint64_t cand_hash_c(const double t[6]) {
-    uint64_t l[6];
-#pragma unroll 1
-    for (int i = 0; i < 6; i++) l[i] = hash_double(t[i]);
-    return tuple_hash6(l);
-}
+// rot_dims_c, cand_tuple, hash_double_call, cand_hash_c, cand_equal and the set emulation (PCTC_CANDIDATES_BODY): pct_cand_c.cuh
 
 __device__ __noinline__ void draw_item_c(const CParams &p, int e, CHdr &h) {
     const uint64_t gid = (uint64_t)(p.env_id_base + e), d = (uint64_t)h.draw_pos;
@@ -363,17 +337,6 @@ __global__ void __launch_bounds__(64) pctc_apply_kernel(const CParams p) {
 }
 
 // ================= K2: candidates in CPython-set order (C:space.py:531-568) =================
-// Table slots are 32 bits: candidate code | 16-bit tag (the top bits of the tuple hash — CPython compares the stored hash before the keys, setobject.c).
-// A probe rejects a non-matching slot on the tag alone; the exact 6-double comparison (tuples rebuilt from the two codes) runs only on a tag match,
-// i.e. practically only for true duplicates.  Round 1 rebuilt and compared the tuple of EVERY probed slot and broadcast the six doubles of every
-// inserted key through shuffles (a large share of this kernel's instructions went to _Py_HashDouble's frexp loop — now an integer rotation,
-// pct_pyhash.cuh — and to shuffles).
-__device__ __forceinline__ bool cand_equal(uint16_t a, uint16_t b, const double (*ems)[6], const double nb[3]) {
-    double u[6], v[6];
-    cand_tuple(a, ems, nb, u);
-    cand_tuple(b, ems, nb, v);
-    return u[0] == v[0] && u[1] == v[1] && u[2] == v[2] && u[3] == v[3] && u[4] == v[4] && u[5] == v[5];
-}
 
 __global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
     __shared__ uint32_t tabA[CC_TAB], tabB[512];
@@ -391,173 +354,7 @@ __global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
     const CHdr &h = ev->h;
     const double nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
     const int R = p.setting == 2 ? 6 : 2, n_ems = h.n_ems;
-    constexpr uint32_t EMPTY = 0xFFFFFFFFu;
-    uint32_t *tab = tabA;
-    uint32_t mask = 7;
-    int fill = 0;
-    if (lane < 8) tab[lane] = EMPTY;
-    __syncwarp();
-    const int raw = n_ems * R * 4;
-    bool stop = false;
-#pragma unroll 1
-    for (int base = 0; base < raw && !stop; base += 32) {
-        const int r = base + lane;
-        bool valid = false;
-        uint64_t hash = 0;
-        uint16_t code = 0;
-        // The four corners of one (EMS, orientation) are four adjacent lanes and their 6-tuples draw on ten distinct coordinates (x: m0, m0 + sx, m3 - sx,
-        // m3; y alike; z: m2, m2 + sz): every lane hashes two or three of them (_Py_HashDouble, the expensive part) and the group exchanges the results,
-        // instead of six hashes per lane.  Same expressions as cand_tuple, so the same bits.
-        uint64_t h0 = 0, h1 = 0, h2 = 0;
-        const int q = r & 3;
-        if (r < raw) {
-            const int er = r >> 2, rot = er % R, ei = er / R;
-            double sx, sy, sz;
-            if (rot_dims_c(nb, rot, sx, sy, sz)) {
-                const double *m = ev->ems[ei];
-                if (m[3] - m[0] + 1e-6 >= sx && m[4] - m[1] + 1e-6 >= sy && m[5] - m[2] + 1e-6 >= sz) {
-                    valid = true;
-                    code = (uint16_t)((ei << 5) | (rot << 2) | q);
-                    double v0, v1, v2 = 0;
-                    if (q == 0) { v0 = m[0]; v1 = m[0] + sx; v2 = m[2]; }
-                    else if (q == 1) { v0 = m[3] - sx; v1 = m[3]; v2 = m[2] + sz; }
-                    else if (q == 2) { v0 = m[1]; v1 = m[1] + sy; }
-                    else { v0 = m[4] - sy; v1 = m[4]; }
-                    h0 = hash_double_call(v0);
-                    h1 = hash_double_call(v1);
-                    if (q < 2) h2 = hash_double_call(v2);
-                }
-            }
-        }
-        {
-            const int gb = lane & ~3, lx = gb + (q & 1), ly = gb + 2 + (q >> 1);
-            uint64_t l6[6];
-            l6[0] = __shfl_sync(FULL, h0, lx); l6[3] = __shfl_sync(FULL, h1, lx);
-            l6[1] = __shfl_sync(FULL, h0, ly); l6[4] = __shfl_sync(FULL, h1, ly);
-            l6[2] = __shfl_sync(FULL, h2, gb); l6[5] = __shfl_sync(FULL, h2, gb + 1);
-            if (valid) hash = tuple_hash6(l6);
-        }
-        // already present? (read-only probe; present keys sit on their own probe sequence)
-        if (valid) {
-            const uint32_t tag = (uint32_t)(hash >> 48);
-            uint64_t perturb = hash;
-            uint32_t i = (uint32_t)hash & mask;
-            bool open = true;
-            while (open) {
-                const int probes = (i + 9 <= mask) ? 9 : 0;
-                for (int j = 0; j <= probes; j++) {
-                    const uint32_t s = tab[i + j];
-                    if (s == EMPTY) { open = false; break; }
-                    if ((s >> 16) == tag && cand_equal((uint16_t)s, code, ev->ems, nb)) { open = false; valid = false; break; }
-                }
-                perturb >>= 5;
-                i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;
-            }
-        }
-        // the new keys of this chunk go through the order-defining insertion in lane (= reference) order: staged in shared memory and inserted by
-        // lane 0 with a scalar set_add_entry (3x fewer warp instructions than a warp-uniform probe with shuffles, as in the discrete kernel);
-        // an equal tuple staged by an earlier lane of the same chunk is found by the tag + exact comparison like any other present key
-        const uint32_t vm = __ballot_sync(FULL, valid);
-        const int n_new = __popc(vm);
-        if (valid) {
-            const int pos = __popc(vm & ((1u << lane) - 1));
-            stg_h[pos] = hash;
-            stg_c[pos] = code;
-        }
-        __syncwarp();
-        int done = 0;
-#pragma unroll 1
-        while (done < n_new && !stop) {
-            int upto = n_new;
-            if (lane == 0) {
-#pragma unroll 1
-                for (int t = done; t < n_new; t++) {
-                    const uint64_t hk = stg_h[t];
-                    const uint16_t ck = stg_c[t];
-                    const uint32_t tagk = (uint32_t)(hk >> 48);
-                    uint64_t perturb = hk;
-                    uint32_t i = (uint32_t)hk & mask;
-                    int state = 0;
-#pragma unroll 1
-                    while (!state) {
-                        const int probes = (i + 9 <= mask) ? 9 : 0;
-#pragma unroll 1
-                        for (int j = 0; j <= probes; j++) {
-                            const uint32_t sl = tab[i + j];
-                            if (sl == EMPTY) { tab[i + j] = (tagk << 16) | ck; state = 1; break; }
-                            if ((sl >> 16) == tagk && cand_equal((uint16_t)sl, ck, ev->ems, nb)) { state = 2; break; }
-                        }
-                        perturb >>= 5;
-                        i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;
-                    }
-                    if (state == 1 && (uint32_t)(++fill) * 5 >= mask * 3) { upto = t + 1; break; }
-                }
-            }
-            upto = __shfl_sync(FULL, upto, 0);
-            fill = __shfl_sync(FULL, fill, 0);
-            done = upto;
-            __syncwarp();
-            if ((uint32_t)fill * 5 >= mask * 3) {
-                uint32_t newsize = 8;
-                while (newsize <= (uint32_t)fill * 4) newsize <<= 1;
-                if (newsize > CC_TAB) { fl |= PCT_FLAG_CAND_OVERFLOW; stop = true; break; }
-                uint32_t *nt = (tab == tabA) ? tabB : tabA;
-                for (uint32_t t = lane; t < newsize; t += 32) nt[t] = EMPTY;
-                __syncwarp();
-#pragma unroll 1
-                for (uint32_t b2 = 0; b2 <= mask; b2 += 32) {  // set_table_resize: re-insert in slot order (set_insert_clean: no comparisons)
-                    const uint32_t sidx = b2 + lane;
-                    const uint32_t c2 = sidx <= mask ? tab[sidx] : EMPTY;
-                    const uint32_t em = __ballot_sync(FULL, c2 != EMPTY);
-                    if (c2 != EMPTY) {
-                        double u[6];
-                        cand_tuple((uint16_t)c2, ev->ems, nb, u);
-                        const int pos = __popc(em & ((1u << lane) - 1));
-                        rs_h[pos] = cand_hash_c(u);
-                        rs_c[pos] = c2;
-                    }
-                    __syncwarp();
-                    if (lane == 0) {
-                        const int m2 = __popc(em);
-#pragma unroll 1
-                        for (int t = 0; t < m2; t++) {
-                            uint64_t pt = rs_h[t];
-                            uint32_t ii = (uint32_t)pt & (newsize - 1);
-                            bool placed = false;
-#pragma unroll 1
-                            while (!placed) {
-                                const int pr = (ii + 9 <= newsize - 1) ? 9 : 0;
-                                for (int j = 0; j <= pr; j++)
-                                    if (nt[ii + j] == EMPTY) { nt[ii + j] = rs_c[t]; placed = true; break; }
-                                pt >>= 5;
-                                ii = (uint32_t)((uint64_t)ii * 5 + 1 + pt) & (newsize - 1);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                }
-                tab = nt;
-                mask = newsize - 1;
-            }
-        }
-        __syncwarp();
-    }
-    __syncwarp();
-    int cnt = 0;
-#pragma unroll 1
-    for (uint32_t b2 = 0; b2 <= mask; b2 += 32) {
-        const uint32_t s = b2 + lane;
-        const uint32_t c2 = s <= mask ? tab[s] : EMPTY;
-        const uint32_t em = __ballot_sync(FULL, c2 != EMPTY);
-        if (c2 != EMPTY) ev->cand[cnt + __popc(em & ((1u << lane) - 1))] = (uint16_t)c2;
-        cnt += __popc(em);
-    }
-    __syncwarp();
-    if (p.shuffle) {  // scratch: the GENEMS temp list (24 KB, idle between apply kernels): keys at 0, permuted codes at 10 KB
-        static_assert(sizeof(ev->ems_tmp) >= 10240 + sizeof(ev->cand), "shuffle scratch fits");
-        shuffle_candidates<uint16_t>(ev->cand, cnt, (uint64_t *)ev->ems_tmp, (uint16_t *)((char *)ev->ems_tmp + 10240), p.seed, (uint64_t)(p.env_id_base + e),
-                                     (uint64_t)h.draw_pos, lane);
-    }
+    PCTC_CANDIDATES_BODY
     if (p.walk.walkq) {
         // ---- classify (round 2): drop_box_virtual's bounds / resting height (C:space.py:380-398) on pre-rounded box rectangles, supports + exact
         // quick reject for the placements that rest on boxes; the stability walks of all envs go to one pool (pctc_walk_light / pctc_walk kernels) ----

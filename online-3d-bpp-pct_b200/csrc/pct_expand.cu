@@ -1,0 +1,312 @@
+// Leaf expansion of caller-given items, read-only (pct_expand_items, include/pct_b200.h): for row r and item j, the leaf rows that
+// get_possible_position() (D:bin3D.py:100-136, C:bin3D.py) produces for that item on env env[r] in its current state.
+//
+// One block of EXPAND_THREADS per row, which takes the row's k items in turn.  Per item:
+//   warp 0    the ordered candidate list with the candidates kernel's own routines (build_candidates and the EV / EP / CP / FC generators,
+//             pct_cand.cuh; PCTC_CANDIDATES_BODY, pct_cand_c.cuh), then the keyed shuffle, into the env's candidate scratch;
+//   block     one thread per candidate in EXPAND_THREADS chunks: bounds, resting height and stability_check<false>, the code of the step's
+//             block-mode feasibility kernel; ordered compaction of the first `nl` feasible candidates;
+//   out       the leaf rows as the observation carries them, and the info record pct_set_items would write.
+// The pooled walk stage is not used: its pools and counters belong to the step.
+//
+// Nothing the env keeps is written.  Scratch: the transient fields every step writes before it reads them — discrete cold->cand / raw
+// (candidate list, generator output, shuffle keys) and cold->big (under the block's lock); continuous ev->cand / ems_tmp / big.  Capacity
+// flags raised by an expansion go to its own info record only.  The envs of one launch are distinct (caller's contract): the scratch is per env.
+#include "pct_common.cuh"
+#include "pct_stability.cuh"
+#include "pct_kernels.h"
+#include "pct_geom.cuh"
+#include "pct_rot.cuh"
+#include "pct_cand.cuh"
+#include "pct_geom_continuous.cuh"
+#include "pct_continuous.cuh"
+#include "pct_cand_c.cuh"
+
+namespace pct {
+
+constexpr int EXPAND_THREADS = 64;  // two warps: the compaction below adds up the ballots of warps 0 and 1
+
+// shared memory of one discrete block: the staged record (TMA), the set emulation's tables (the 2048-slot stage included), the leaves
+template <typename SlotT>
+struct ExpandSmD {
+    DEnvHot hot;
+    SlotT tabA[TAB_A], tabB[TAB_B];
+    SetStage stg;
+    int16_t leaf[NL_MAX][6];
+    alignas(16) Stack4 st[EDGE_STAGE];
+    alignas(16) double poly[POLY_STAGE * 2];
+    uint64_t mbar;
+    RotTab rt;
+    int lock, fl, n_cand;
+    uint32_t wb[2];
+};
+
+// zero rows and a zero record for a row whose env index is outside the handle
+template <typename OT>
+__device__ __forceinline__ void expand_zero_row(const ExpandParams &x, int nl, size_t row, int tid) {
+    OT *out = (OT *)x.leaves + row * (size_t)nl * 9;
+    for (size_t f = tid; f < (size_t)x.k * nl * 9; f += EXPAND_THREADS) out[f] = 0;
+    if (x.info)
+        for (int j = tid; j < x.k; j += EXPAND_THREADS) x.info[row + j] = pct_step_info{};
+}
+
+template <typename OT, bool STAB, typename SlotT>
+__global__ void __launch_bounds__(EXPAND_THREADS) pct_expand_kernel(const DParams p, const ExpandParams x) {
+    constexpr int KB = sizeof(SlotT) == 2 ? 4 : 8;
+    __shared__ __align__(16) ExpandSmD<SlotT> s;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, r = blockIdx.x, K = x.k, nl = p.nl;
+    const int e = x.env ? x.env[r] : r;
+    const size_t row = (size_t)r * K;
+    if (e < 0 || e >= p.n_envs) { expand_zero_row<OT>(x, nl, row, tid); return; }
+    DEnvHot *hot = &s.hot;
+    DEnvCold *cold = p.cold + e;
+    if (tid == 0) {
+        s.lock = 0;
+        mbar_init(&s.mbar, 1);
+        fence_proxy_async();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        mbar_expect_tx(&s.mbar, (uint32_t)sizeof(DEnvHot));
+        tma_load_1d(hot, p.hot + e, (uint32_t)sizeof(DEnvHot), &s.mbar);
+    }
+    mbar_wait(&s.mbar, 0);
+    __syncthreads();
+    const DHdr &h = hot->h;
+    if (STAB && h.n_edge > 0) {  // the first load edges and polygon vertices (second phase of the same mbarrier)
+        const uint32_t bytes = (uint32_t)min(h.n_edge, EDGE_STAGE) * (uint32_t)sizeof(Stack4);
+        const uint32_t pbytes = (uint32_t)min(h.n_poly, POLY_STAGE) * 16u;
+        if (tid == 0) {
+            mbar_expect_tx(&s.mbar, bytes + pbytes);
+            tma_load_1d(s.st, cold->e_st, bytes, &s.mbar);
+            if (pbytes) tma_load_1d(s.poly, cold->poly, pbytes, &s.mbar);
+        }
+        mbar_wait(&s.mbar, 1);
+    }
+    __syncthreads();
+    const int n_box = h.n_box, R = p.setting == 2 ? 6 : 2;
+    GeomD g{hot->box, n_box, p.setting == 3 ? cold->density : nullptr};
+    EdgePool pool{hot->e_lower, hot->e_next, hot->e_off, hot->first_in, hot->last_in, cold->e_st, s.st, h.n_edge,
+                  hot->poly_off, &cold->poly[0][0], s.poly, h.n_poly};
+    SlotT *const out = (SlotT *)cold->cand;
+    const RotTab *rt = &s.rt;
+#pragma unroll 1
+    for (int j = 0; j < K; j++) {
+        const int32_t *it = (const int32_t *)x.items + (row + j) * 3;
+        const double den = x.density ? x.density[row + j] : h.next_den;
+        if (warp == 0) {
+            // ---- the candidates kernel's list for this item (pct_candidates_kernel) ----
+            const int nb3[3] = {min(max(it[0], 0), 255), min(max(it[1], 0), 255), min(max(it[2], 0), 255)};  // as pct_set_items clamps
+            if (lane == 0) make_rot_tab(nb3, R, s.rt);
+            __syncwarp();
+            SlotT *cand = nullptr;
+            int fl = 0, n_cand;
+            if (p.lnes == 0) {
+                n_cand = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, cand, lane, fl);
+            } else {
+                uint32_t *raw = cold->raw;
+                int n_raw;
+                if (p.lnes == 4) n_raw = gen_full_coord<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, raw, lane, fl);
+                else if (p.lnes == 1) n_raw = gen_event_point<KB>(rt, R, p.W, p.L, raw, lane);
+                else n_raw = gen_level_points<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, p.lnes == 2, raw, lane, fl);
+                if (n_raw == -2) {  // empty bin under EP / CP: the reference's 2-element list (D:space.py:700-701)
+                    if (lane < 2) out[lane] = (SlotT)key_pack<KB>(0, 0, 0, rt->canon[lane]);
+                    n_cand = 2;
+                    cand = out;
+                } else
+                    n_cand = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, cand, lane, fl, raw, n_raw);
+            }
+            if (cand != out)
+                for (int t = lane; t < n_cand; t += 32) out[t] = cand[t];
+            __syncwarp();
+            if (p.shuffle)  // same keys (seed, global env id, draw_pos) and scratch (cold->raw + cold->tab_big) as the candidates kernel
+                shuffle_candidates<SlotT>(out, n_cand, (uint64_t *)cold->raw, (SlotT *)((char *)cold->raw + 10240), p.seed, (uint64_t)(p.env_id_base + e),
+                                          (uint64_t)h.draw_pos, lane);
+            if (lane == 0) { s.n_cand = n_cand; s.fl = fl; }
+        }
+        __syncthreads();
+        // ---- get_possible_position: first `nl` feasible candidates in order (the step's block-mode feasibility kernel) ----
+        const int n_cand = s.n_cand;
+        int n_leaf = 0, fl = 0;
+#pragma unroll 1
+        for (int base = 0; base < n_cand && n_leaf < nl; base += EXPAND_THREADS) {
+            const int c = base + tid;
+            bool feas = false;
+            int xs = 0, ys = 0, zs = 0, rot = 0, sx = 0, sy = 0, sz = 0;
+            if (c < n_cand) {
+                key_unpack<KB>(out[c], xs, ys, zs, rot);
+                sx = rt->d[rot][0]; sy = rt->d[rot][1]; sz = rt->d[rot][2];
+                const int mh = rest_height(hot->box, 0, n_box, 1, xs, ys, xs + sx, ys + sy);
+                if (xs + sx > p.W || ys + sy > p.L) feas = false;
+                else if (mh + sz > p.H) feas = false;
+                else if (!STAB || mh == 0) feas = true;
+                else {
+                    NodeD root{xs, ys, mh, sx, sy, sz, (double)(sx * sy * sz) * den};
+                    feas = stability_check<false, GeomD>(g, root, pool, &cold->big, &s.lock, 0, fl) != 0;
+                }
+            }
+            const uint32_t fm = __ballot_sync(FULL, feas);
+            if (lane == 0) s.wb[warp] = fm;
+            __syncthreads();
+            const int before = warp == 1 ? __popc(s.wb[0]) : 0, total = __popc(s.wb[0]) + __popc(s.wb[1]);
+            if (feas) {
+                const int kk = n_leaf + before + __popc(fm & ((1u << lane) - 1));
+                if (kk < nl) {
+                    s.leaf[kk][0] = (int16_t)xs; s.leaf[kk][1] = (int16_t)ys; s.leaf[kk][2] = (int16_t)zs;
+                    s.leaf[kk][3] = (int16_t)(xs + sx); s.leaf[kk][4] = (int16_t)(ys + sy); s.leaf[kk][5] = (int16_t)(zs + sz);
+                }
+            }
+            n_leaf += total;
+            __syncthreads();
+        }
+        if (n_leaf > nl) n_leaf = nl;
+        fl = __reduce_or_sync(FULL, fl);
+        if (fl && lane == 0) atomicOr(&s.fl, fl);
+        __syncthreads();
+        // ---- the leaf rows of cur_observation (write_obs) and the record of pct_set_items ----
+        OT *o = (OT *)x.leaves + (row + j) * (size_t)nl * 9;
+#pragma unroll 1
+        for (int f = tid; f < nl * 9; f += EXPAND_THREADS) {
+            const int k = f / 9, col = f - k * 9;
+            OT v = 0;
+            if (k < n_leaf) {
+                if (col < 5) v = (OT)s.leaf[k][col];
+                else if (col == 5) v = (OT)p.H;
+                else if (col == 8) v = 1;
+            }
+            o[f] = v;
+        }
+        if (tid == 0 && x.info) {
+            pct_step_info info{};
+            info.counter = n_box;
+            info.flags = h.flags | s.fl;
+            info.n_leaf = n_leaf; info.n_cand = n_cand; info.n_ems = h.n_ems;
+            x.info[row + j] = info;
+        }
+        __syncthreads();  // the next item reuses the rotation table, the leaves and the candidate scratch
+    }
+}
+
+template <typename OT, bool STAB>
+__global__ void __launch_bounds__(EXPAND_THREADS) pctc_expand_kernel(const CParams p, const ExpandParams x) {
+    __shared__ uint32_t tabA[CC_TAB], tabB[512];
+    __shared__ uint64_t stg_h[32], rs_h[32];
+    __shared__ uint32_t rs_c[32];
+    __shared__ uint16_t stg_c[32];
+    __shared__ double leaf[NL_MAX][6];
+    __shared__ uint32_t wb[2];
+    __shared__ int lock, s_fl, s_cnt;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, r = blockIdx.x, K = x.k, nl = p.nl;
+    const int e = x.env ? x.env[r] : r;
+    const size_t row = (size_t)r * K;
+    if (e < 0 || e >= p.n_envs) { expand_zero_row<OT>(x, nl, row, tid); return; }
+    CEnv *ev = p.env + e;
+    const CHdr &h = ev->h;
+    if (tid == 0) lock = 0;
+    const int R = p.setting == 2 ? 6 : 2, n_ems = h.n_ems, n_box = h.n_box;
+    GeomC g{ev->box, ev->den, n_box};
+    EdgePool pool{ev->e_lower, ev->e_next, ev->e_off, ev->first_in, ev->last_in, ev->e_st, ev->e_st, h.n_edge,
+                  ev->poly_off, &ev->poly[0][0], &ev->poly[0][0], h.n_poly};
+#pragma unroll 1
+    for (int j = 0; j < K; j++) {
+        const double *it = (const double *)x.items + (row + j) * 3;
+        const double nb[3] = {it[0], it[1], it[2]};
+        const double den = x.density ? x.density[row + j] : h.next_den;
+        if (warp == 0) {
+            int fl = 0;
+            PCTC_CANDIDATES_BODY
+            if (lane == 0) { s_cnt = cnt; s_fl = fl; }
+        }
+        __syncthreads();
+        // ---- get_possible_position (the step's block-mode feasibility kernel, pctc_feas_emit_kernel) ----
+        const int n_cand = s_cnt;
+        int n_leaf = 0, fl = 0;
+#pragma unroll 1
+        for (int base = 0; base < n_cand && n_leaf < nl; base += EXPAND_THREADS) {
+            const int c = base + tid;
+            bool feas = false;
+            double t6[6] = {0, 0, 0, 0, 0, 0};
+            if (c < n_cand) {
+                cand_tuple(ev->cand[c], ev->ems, nb, t6);
+                const double x6 = t6[3] - t6[0], y6 = t6[4] - t6[1], z6 = t6[5] - t6[2], lx = t6[0], ly = t6[1];
+                bool chk = !(lx + x6 - 1e-6 > p.W || ly + y6 - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
+                double mh = rest_height_c(ev->box, 0, n_box, 1, lx, ly, lx + x6, ly + y6);
+                if (mh < 0) mh = 0.0;
+                if (mh + z6 - 1e-6 > p.H) chk = false;
+                if (!chk) feas = false;
+                else if (!STAB || fabs(mh) < 1e-6) feas = true;
+                else {
+                    NodeC root{lx, ly, mh, x6, y6, z6, x6 * y6 * z6 * den};
+                    feas = stability_check<false, GeomC>(g, root, pool, &ev->big, &lock, 0, fl) != 0;
+                }
+            }
+            const uint32_t fm = __ballot_sync(FULL, feas);
+            if (lane == 0) wb[warp] = fm;
+            __syncthreads();
+            const int before = warp == 1 ? __popc(wb[0]) : 0, total = __popc(wb[0]) + __popc(wb[1]);
+            if (feas) {
+                const int kk = n_leaf + before + __popc(fm & ((1u << lane) - 1));
+                if (kk < nl)
+                    for (int t = 0; t < 6; t++) leaf[kk][t] = t6[t];
+            }
+            n_leaf += total;
+            __syncthreads();
+        }
+        if (n_leaf > nl) n_leaf = nl;
+        fl = __reduce_or_sync(FULL, fl);
+        if (fl && lane == 0) atomicOr(&s_fl, fl);
+        __syncthreads();
+        OT *o = (OT *)x.leaves + (row + j) * (size_t)nl * 9;
+#pragma unroll 1
+        for (int f = tid; f < nl * 9; f += EXPAND_THREADS) {  // write_obs_c's leaf rows
+            const int k = f / 9, col = f - k * 9;
+            double v = 0;
+            if (k < n_leaf) {
+                if (col < 5) v = leaf[k][col];
+                else if (col == 5) v = p.H;
+                else if (col == 8) v = 1;
+            }
+            o[f] = (OT)v;
+        }
+        if (tid == 0 && x.info) {
+            pct_step_info info{};
+            info.counter = n_box;
+            info.flags = h.flags | s_fl;
+            info.n_leaf = n_leaf; info.n_cand = n_cand; info.n_ems = n_ems;
+            x.info[row + j] = info;
+        }
+        __syncthreads();
+    }
+}
+
+template <typename OT>
+static void expand_discrete(const DParams &p, const ExpandParams &x, cudaStream_t st) {
+    const bool stab = p.setting != 2, small = p.W <= 16 && p.L <= 16 && p.H <= 16;  // the candidate key width of the step (launch_s)
+    if (small) {
+        if (stab) pct_expand_kernel<OT, true, uint16_t><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+        else pct_expand_kernel<OT, false, uint16_t><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+    } else {
+        if (stab) pct_expand_kernel<OT, true, uint32_t><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+        else pct_expand_kernel<OT, false, uint32_t><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+    }
+}
+
+cudaError_t launch_expand_discrete(const DParams &p, const ExpandParams &x, cudaStream_t st) {
+    if (p.obs_f64) expand_discrete<double>(p, x, st);
+    else expand_discrete<float>(p, x, st);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_expand_continuous(const CParams &p, const ExpandParams &x, cudaStream_t st) {
+    const bool stab = p.setting != 2;
+    if (p.obs_f64) {
+        if (stab) pctc_expand_kernel<double, true><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+        else pctc_expand_kernel<double, false><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+    } else {
+        if (stab) pctc_expand_kernel<float, true><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+        else pctc_expand_kernel<float, false><<<x.n, EXPAND_THREADS, 0, st>>>(p, x);
+    }
+    return cudaGetLastError();
+}
+
+}  // namespace pct

@@ -291,6 +291,17 @@ cudaError_t launch_preview_discrete(const DParams &p, const ItemParams &ip, cuda
 // the item kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
 cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
 
+// read-only leaf expansion of caller-given items (pct_expand.cu): row r expands k items on env env[r]
+struct ExpandParams {
+    const int32_t *env;      // [n] env of row r, nullptr: env r
+    int n, k;
+    const void *items;       // n x k x 3 sizes, int32 (discrete) / float64 (continuous)
+    const double *density;   // n x k, nullptr: the env's current item density
+    void *leaves;            // n x k x nl x 9 leaf rows, the observation dtype
+    pct_step_info *info;     // n x k records, or nullptr
+};
+cudaError_t launch_expand_discrete(const DParams &p, const ExpandParams &x, cudaStream_t st);
+
 // per-env reset (pct_reset.cu; continuous: pct_continuous.cu): env e resets iff mask[e] != 0 (mask non-null) or e is one of env[0..n)
 struct ResetParams {
     const int32_t *env;
@@ -332,6 +343,7 @@ cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool a
 cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st);
 cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st);
 cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st);
+cudaError_t launch_expand_continuous(const CParams &p, const ExpandParams &x, cudaStream_t st);
 cudaError_t launch_queries_continuous(const CParams &p, const QParams &q, cudaStream_t st);
 cudaError_t launch_heuristic_continuous(const CParams &p, const HParamsC &hp, cudaStream_t st);
 cudaError_t launch_policy_random_continuous(const CEnv *env, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
