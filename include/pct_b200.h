@@ -57,7 +57,10 @@ enum pct_item_mode {
 /* Per-environment flag bits reported in pct_step_info.flags (sticky until the env resets). */
 enum pct_env_flags {
     PCT_FLAG_BOX_OVERFLOW = 1,      /* more than internal_node_holder boxes (IndexError in D:space.py:385) */
-    PCT_FLAG_BAD_ACTION = 2,        /* leaf row does not match the item (ValueError in D:bin3D.py:144-145) */
+    PCT_FLAG_BAD_ACTION = 2,        /* the reference raises on this action: a leaf row that does not match the item (ValueError in
+                                       D:bin3D.py:144-145), or, discrete, a footprint whose slice plain[lx:lx+x, ly:ly+y] is empty under
+                                       Python slice rules (np.max of an empty array in D:space.py:354-355; e.g. lx >= max(W, L), or
+                                       plain[-1:1]).  The episode ends as for any failed placement, with the same counter and ratio */
     PCT_FLAG_EMS_OVERFLOW = 4,      /* EMS list exceeded the fixed capacity                                */
     PCT_FLAG_CAND_OVERFLOW = 8,     /* candidate set exceeded the fixed capacity                           */
     PCT_FLAG_EDGE_OVERFLOW = 16,    /* support-edge pool exceeded the fixed capacity                       */
@@ -164,7 +167,8 @@ int pct_reset(pct_handle h, void *d_obs, void *stream);
  * its reset observation; reward/done/info are the terminal ones).
  *   d_actions  : n_envs x 9 leaf rows (float32 if action_f64==0 else float64), or NULL
  *   d_leaf_idx : n_envs int32 indices into the previous observation's leaf rows (fast path), or NULL;
- *                an index >= the env's n_leaf selects the all-zero row.  Exactly one of the two is non-NULL.
+ *                an index >= the env's n_leaf, and any NEGATIVE index (no Python-style wrap to the last rows), selects the all-zero
+ *                row, which places the item unrotated at (0, 0).  Exactly one of the two is non-NULL.
  *   d_reward   : n_envs float32;  d_done: n_envs uint8;  d_info: n_envs pct_step_info (may be NULL)
  * Observation buffer contract (delta rows, default; PCT_B200_OBS_DELTA=0 restores full rewrites): 75 % of the (internal + leaf + 1) x 9
  * observation is zero padding and the internal-node rows are append-only within an episode, so when a call receives the SAME d_obs pointer

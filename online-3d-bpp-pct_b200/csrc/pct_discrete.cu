@@ -454,6 +454,12 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kerne
                 if (lane == 0) h.flags |= PCT_FLAG_BOX_OVERFLOW;
             }
         }
+        if (lane == 0 && !bad && (lx < 0 || ly < 0 || lx >= maxax || ly >= maxax)) {
+            // np.max(plain[lx:lx + x, ly:ly + y]) raises on an empty slice of the max(W, L)-square plain (D:space.py:354-355).  Unlike the
+            // oracle's guard, no x <= 0 / y <= 0 term: when !bad, x and y are sides of the item (>= 1), so only the start can empty the slice
+            auto py = [maxax](int i) { return i < 0 ? max(i + maxax, 0) : min(i, maxax); };  // Python's clamp of a slice bound
+            bad = py(lx) >= py(lx + x) || py(ly) >= py(ly + y);
+        }
         if (bad && lane == 0) h.flags |= PCT_FLAG_BAD_ACTION;
         __syncwarp();
         const double binvol = (double)(p.W * p.L * p.H);
