@@ -33,7 +33,14 @@ struct SetStage {  // per-warp staging of (hash, key) pairs for the serial inser
     uint32_t k[32];
 };
 
-// returns the candidate count; the ordered keys end up at the start of `out`.
+// The ordered list: `n` keys at `keys` (one of the tables), `flags` the PCT_FLAG_* bits raised.  Results come back by value: an output
+// argument taken by reference would pin the caller's variable to the stack frame.
+template <typename SlotT>
+struct CandList {
+    SlotT *keys;
+    int n, flags;
+};
+
 // Inserting a key that is already in the set is a no-op, so only FIRST occurrences have to go through the
 // order-defining serial insertion: every lane first looks its key up in the current table (read-only, the
 // lookup of a present key follows exactly the probe sequence that placed it), duplicates inside the 32-wide
@@ -42,13 +49,13 @@ struct SetStage {  // per-warp staging of (hash, key) pairs for the serial inser
 // set_insert_clean (the kernel is instruction-issue bound: a one-lane scalar loop costs ~3x fewer warp
 // instructions than a ballot-based warp-wide probe).  Resizes re-hash the old table in parallel, 32 slots at a time.
 template <typename SlotT>
-__device__ __noinline__ int build_candidates(const int16_t (*ems)[6], int n_ems, const RotTab *rt, int R, SlotT *tabA, SlotT *tabB, SlotT *tabBig,
-                                             SetStage *stg, SlotT *&out, int lane, int &flags, const uint32_t *raw_keys = nullptr, int n_raw = 0) {
+__device__ __noinline__ CandList<SlotT> build_candidates(const int16_t (*ems)[6], int n_ems, const RotTab *rt, int R, SlotT *tabA, SlotT *tabB, SlotT *tabBig,
+                                                         SetStage *stg, int lane, const uint32_t *raw_keys = nullptr, int n_raw = 0) {
     constexpr int BITS = sizeof(SlotT) == 2 ? 4 : 8;
     constexpr SlotT EMPTY = (SlotT)~(SlotT)0;
     SlotT *tab = tabA;
     uint32_t mask = 7;
-    int fill = 0;
+    int fill = 0, flags = 0;
     if (lane < 8) tab[lane] = EMPTY;
     __syncwarp();
     const int raw = raw_keys ? n_raw : n_ems * R * 4;  // raw_keys: insertion sequence produced by an EV / EP / CP / FC generator
@@ -174,18 +181,21 @@ __device__ __noinline__ int build_candidates(const int16_t (*ems)[6], int n_ems,
         cnt += __popc(em);
         __syncwarp();
     }
-    out = tab;
-    return cnt;
+    return CandList<SlotT>{tab, cnt, flags};
 }
 
 // ---- the other leaf-node expansion schemes (D:bin3D.py:101-112): generators of the set-insertion sequence --------------
 constexpr int RAW_MAX = 2048;
 
+struct RawList {  // a generator's insertion sequence: `n` keys in the caller's raw buffer, `flags` the PCT_FLAG_* bits raised
+    int n, flags;
+};
+
 // FullCoord (D:space.py:573-610): every cell x valid rotation with lz = height of the cell, rot-major / lx / ly order
 template <int BITS>
-__device__ __noinline__ int gen_full_coord(const int16_t (*box)[6], int n_box, const RotTab *rt, int R, int W, int L, int H, uint32_t *raw,
-                                           int lane, int &flags) {
-    int n = 0;
+__device__ __noinline__ RawList gen_full_coord(const int16_t (*box)[6], int n_box, const RotTab *rt, int R, int W, int L, int H, uint32_t *raw,
+                                               int lane) {
+    int n = 0, flags = 0;
     const int cells = W * L;
 #pragma unroll 1
     for (int rot = 0; rot < R; rot++) {
@@ -210,7 +220,7 @@ __device__ __noinline__ int gen_full_coord(const int16_t (*box)[6], int n_box, c
     }
     if (n > RAW_MAX) { flags |= PCT_FLAG_CAND_OVERFLOW; n = RAW_MAX; }
     __syncwarp();
-    return n;
+    return RawList{n, flags};
 }
 
 // EventPoint (D:space.py:613-693) as the reference actually behaves: GENEMS (which maintains EMS and ZMAP) only runs for
@@ -240,10 +250,10 @@ __device__ __noinline__ int gen_event_point(const RotTab *rt, int R, int W, int 
 // above k; points new w.r.t. the previous level x rotations.  Small serial algorithms over <= 80 boxes: lane 0 runs them.
 // Returns -2 for the empty-bin special case (two hard-coded placements, a list, no set).
 template <int BITS>
-__device__ __noinline__ int gen_level_points(const int16_t (*box)[6], int n_box, const RotTab *rt, int R, int W, int L, int H, bool ep,
-                                             uint32_t *raw, int lane, int &flags) {
-    if (n_box == 0) return -2;
-    int n = 0;
+__device__ __noinline__ RawList gen_level_points(const int16_t (*box)[6], int n_box, const RotTab *rt, int R, int W, int L, int H, bool ep,
+                                                 uint32_t *raw, int lane) {
+    if (n_box == 0) return RawList{-2, 0};
+    int n = 0, flags = 0;
     if (lane == 0) {
         int16_t tset[NB_MAX + 1];
         int nt = 0;
@@ -335,7 +345,7 @@ __device__ __noinline__ int gen_level_points(const int16_t (*box)[6], int n_box,
     }
     n = __shfl_sync(FULL, n, 0);
     __syncwarp();
-    return n;
+    return RawList{n, flags};
 }
 
 }  // namespace pct

@@ -42,7 +42,10 @@ namespace pct {
 // A holds the 8 / 128 / 2048 stages, B the 32 / 512 stages.  BIGSM = true keeps the 2048 stage in shared memory
 // (setting 2: 6 orientations, hundreds of candidates per step); BIGSM = false (settings 1/3: <= 306 candidates in
 // practice) keeps A at 128 slots and spills the rare 2048 stage to the env's cold record in HBM, which keeps a warp's
-// share of shared memory at ~5 KB: 32 warps fit in one SM (4096 envs on 132 SMs need ceil(4096 / 132) = 32).
+// share of shared memory at 5056 / 6336 B (16- / 32-bit slots).  4096 envs on 132 SMs run in one resident wave when 32 warps fit in one SM
+// (ceil(4096 / 132) = 32): 16 two-warp blocks take 162 / 203 KB of the 227 KB, and the registers must stay at 64 per thread
+// (K2_MINB = 16; without the bound sm_90a gives the kernel 72-74 and 28 warps fit).  Measured on the H100, the bound loses: the tail of
+// 1.14 waves costs less than the extra instructions at 64 registers, so the default leaves the registers free.
 template <typename SlotT, bool BIGSM>
 struct Lay {
     static constexpr int A_SLOTS = BIGSM ? TAB_A : 128;
@@ -258,10 +261,13 @@ __device__ __forceinline__ long long gtime() { long long t; asm volatile("mov.u6
 #define KT_END(e, k)
 #endif
 #ifndef K1_MINB
-#define K1_MINB 6   // sweep (r1): 168 regs / 6 blocks per SM beats 72 regs / 14 blocks — spills cost more than occupancy gives
+#define K1_MINB 6   // sweeps: B200 (r1) 168 regs / 6 blocks per SM beat 72 regs / 14 blocks; H100 5 ties, 7 and 8 (128 regs, spills) lose 1.4 %
+#endif
+#ifndef K2_MINB
+#define K2_MINB 1   // sweep (H100): 16 (64 regs, one resident wave, see Lay) is 0.8 % slower than no bound (74 regs, 1.14 waves)
 #endif
 #ifndef K3_MINB
-#define K3_MINB 8   // sweep (r1): 128 regs / 8 blocks per SM
+#define K3_MINB 8   // sweep (B200, r1): 128 regs / 8 blocks per SM; the block-mode kernel is not re-measured on the H100
 #endif
 // ---- block scheduling order (longest-processing-time-first) --------------------------------------------------------------------------
 // A launch lasts as long as its slowest block and blocks are dispatched in index order, so the envs with the most expected work (boxes placed
@@ -300,7 +306,7 @@ constexpr int K1_SM_PER_WARP = sizeof(DEnvHot) + EMS_TMP_MAX * 12 + 16 + EDGE_ST
 static_assert(K1_SM_PER_WARP % 16 == 0, "alignment");
 
 template <bool STAB, bool ALIAS = false>
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kernel(const DParams p) {  // ALIAS: see EdgePoolA (the default; PCT_B200_ALIAS=0 selects the snapshot kernel)
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kernel(const __grid_constant__ DParams p) {  // ALIAS: see EdgePoolA (the default; PCT_B200_ALIAS=0 selects the snapshot kernel)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slot = blockIdx.x * WARPS_PER_BLOCK + warp;
@@ -524,8 +530,10 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kerne
 }
 
 // ---- K2: candidate leaves -----------------------------------------------------------------------------------
+// __grid_constant__ (K1, K2, emit): the __noinline__ phases take `const DParams &`; without it every thread first copies the 320 B parameter
+// block into its local-memory frame, so that the reference has an address, and reads the fields back from there.
 template <typename SlotT, bool BIGSM>
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) pct_candidates_kernel(const DParams p) {
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K2_MINB) pct_candidates_kernel(const __grid_constant__ DParams p) {
     typedef Lay<SlotT, BIGSM> LY;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -565,23 +573,27 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) pct_candidates_kernel(co
     if (lane == 0) make_rot_tab(nb3, R, *rt);
     __syncwarp();
     SlotT *cand = nullptr;
-    int fl = 0, n_cand;
+    int fl = 0, n_cand = 0;
     SlotT *out = (SlotT *)cold->cand;
     constexpr int KB = sizeof(SlotT) == 2 ? 4 : 8;
     if (p.lnes == 0) {
-        n_cand = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, tabA, tabB, BIGSM ? tabA : (SlotT *)cold->tab_big, stg, cand, lane, fl);
+        const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, tabA, tabB, BIGSM ? tabA : (SlotT *)cold->tab_big, stg, lane);
+        cand = cl.keys; n_cand = cl.n; fl = cl.flags;
     } else {
         uint32_t *raw = cold->raw;
-        int n_raw;
-        if (p.lnes == 4) n_raw = gen_full_coord<KB>(hot->box, h.n_box, rt, R, p.W, p.L, p.H, raw, lane, fl);
-        else if (p.lnes == 1) n_raw = gen_event_point<KB>(rt, R, p.W, p.L, raw, lane);
-        else n_raw = gen_level_points<KB>(hot->box, h.n_box, rt, R, p.W, p.L, p.H, p.lnes == 2, raw, lane, fl);
-        if (n_raw == -2) {  // empty bin under EP / CP: the reference returns a 2-element LIST (D:space.py:700-701)
+        RawList rl;
+        if (p.lnes == 4) rl = gen_full_coord<KB>(hot->box, h.n_box, rt, R, p.W, p.L, p.H, raw, lane);
+        else if (p.lnes == 1) rl = RawList{gen_event_point<KB>(rt, R, p.W, p.L, raw, lane), 0};
+        else rl = gen_level_points<KB>(hot->box, h.n_box, rt, R, p.W, p.L, p.H, p.lnes == 2, raw, lane);
+        fl = rl.flags;
+        if (rl.n == -2) {  // empty bin under EP / CP: the reference returns a 2-element LIST (D:space.py:700-701)
             if (lane < 2) out[lane] = (SlotT)key_pack<KB>(0, 0, 0, rt->canon[lane]);
             n_cand = 2;
             cand = out;
-        } else
-            n_cand = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, tabA, tabB, BIGSM ? tabA : (SlotT *)cold->tab_big, stg, cand, lane, fl, raw, n_raw);
+        } else {
+            const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, tabA, tabB, BIGSM ? tabA : (SlotT *)cold->tab_big, stg, lane, raw, rl.n);
+            cand = cl.keys; n_cand = cl.n; fl |= cl.flags;
+        }
     }
     if (cand != out)
         for (int t = lane; t < n_cand; t += 32) out[t] = cand[t];
@@ -804,10 +816,10 @@ __global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(co
 // get_possible_position stops at `nl` feasible candidates (D:bin3D.py:117-136); here classification stops once `nl` candidates are KNOWN
 // feasible and the emit kernel takes the first `nl` set bits: the same ordered prefix (walks past the cut are wasted work, not wrong).
 #ifndef WALK_MINB
-#define WALK_MINB 8
+#define WALK_MINB 6   // sweep (H100): 6 (165 regs, no spill) beats 8 (128 regs, the B200 choice) by 1.7 % and 10 (96 regs) by 5 %
 #endif
 #ifndef LIGHT_MINB
-#define LIGHT_MINB 6
+#define LIGHT_MINB 6  // sweep (H100): 4 and 8 both slower
 #endif
 // the discrete domain's side of the walk stage (pct_walks.cuh): hot record for the geometry, cold record for the walk's verdict and scratch
 struct DWalkView {
@@ -845,13 +857,16 @@ __global__ void __launch_bounds__(32 * LIGHT_WARPS, LIGHT_MINB) pct_walk_light_k
 __global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_kernel(const DParams p) { PCT_WALK_CONT_BODY(DWalk, p) }
 __global__ void __launch_bounds__(32 * WALK_WARPS, WALK_MINB) pct_walk_fork_kernel(const DParams p) { walk_fork<DWalk>(p); }
 
-constexpr int EMIT_WARPS = 4;
+#ifndef EMIT_WARPS_N
+#define EMIT_WARPS_N 4
+#endif
+constexpr int EMIT_WARPS = EMIT_WARPS_N;
 constexpr int EMIT_STAGE = sizeof(DHdr) + NB_MAX * 12;  // header + placed boxes: all the observation needs from the hot record
 constexpr int EMIT_SM_PER_WARP = EMIT_STAGE + NL_MAX * 12 + 48;
 static_assert(EMIT_STAGE % 16 == 0 && EMIT_SM_PER_WARP % 16 == 0, "TMA bulk copies move multiples of 16 bytes");
 
 template <typename OT, typename SlotT, bool DELTA>
-__global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const DParams p) {
+__global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const __grid_constant__ DParams p) {
     constexpr int BITS = sizeof(SlotT) == 2 ? 4 : 8;
     __shared__ __align__(16) unsigned char smem[EMIT_WARPS * EMIT_SM_PER_WARP];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;

@@ -100,21 +100,25 @@ __global__ void __launch_bounds__(EXPAND_THREADS) pct_expand_kernel(const DParam
             if (lane == 0) make_rot_tab(nb3, R, s.rt);
             __syncwarp();
             SlotT *cand = nullptr;
-            int fl = 0, n_cand;
+            int fl = 0, n_cand = 0;
             if (p.lnes == 0) {
-                n_cand = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, cand, lane, fl);
+                const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, lane);
+                cand = cl.keys; n_cand = cl.n; fl = cl.flags;
             } else {
                 uint32_t *raw = cold->raw;
-                int n_raw;
-                if (p.lnes == 4) n_raw = gen_full_coord<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, raw, lane, fl);
-                else if (p.lnes == 1) n_raw = gen_event_point<KB>(rt, R, p.W, p.L, raw, lane);
-                else n_raw = gen_level_points<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, p.lnes == 2, raw, lane, fl);
-                if (n_raw == -2) {  // empty bin under EP / CP: the reference's 2-element list (D:space.py:700-701)
+                RawList rl;
+                if (p.lnes == 4) rl = gen_full_coord<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, raw, lane);
+                else if (p.lnes == 1) rl = RawList{gen_event_point<KB>(rt, R, p.W, p.L, raw, lane), 0};
+                else rl = gen_level_points<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, p.lnes == 2, raw, lane);
+                fl = rl.flags;
+                if (rl.n == -2) {  // empty bin under EP / CP: the reference's 2-element list (D:space.py:700-701)
                     if (lane < 2) out[lane] = (SlotT)key_pack<KB>(0, 0, 0, rt->canon[lane]);
                     n_cand = 2;
                     cand = out;
-                } else
-                    n_cand = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, cand, lane, fl, raw, n_raw);
+                } else {
+                    const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, lane, raw, rl.n);
+                    cand = cl.keys; n_cand = cl.n; fl |= cl.flags;
+                }
             }
             if (cand != out)
                 for (int t = lane; t < n_cand; t += 32) out[t] = cand[t];

@@ -65,7 +65,7 @@ struct pct_env_batch {
     bool walk_fork = false;            // PCT_B200_WALK=fork: fork-join continuation kernel (pct_walkq.cuh) instead of the sequential one — measured equal-to-slower (DESIGN.md section 5), kept as an opt-in
     int walk_blocks = 6;               // its blocks per SM (PCT_B200_WALK_BLOCKS)
     int walk_keep = 264;               // its warps that stay as helpers for forked pieces: two per SM of the H100 (PCT_B200_WALK_KEEP)
-    int walk_lanes_tall = 4;           // ... of the tall walks (resting height >= 0.6 H: the longest chains), PCT_B200_WALK_LANES_TALL
+    int walk_lanes_tall = 4;           // ... of the tall walks (resting height >= 0.6 H: the longest chains), PCT_B200_WALK_LANES_TALL (H100 sweep: DESIGN.md section 16)
     int walk_lanes = 16;               // continuations per warp of pct_walk_kernel (PCT_B200_WALK_LANES; few long serial chains: more warps beat fuller warps)
     bool lpt = false;
     int prof_on = 0;

@@ -99,7 +99,7 @@ __device__ __forceinline__ void walk_light(const typename T::Params &p) {
 // walk, stage 2: the continuations — every lane starts with the heavy visit its walk stopped at, then runs the general light / heavy state
 // machine to the end of the walk.  Only `walk_lanes` lanes of a warp carry a walk (default 16; 4 for the tall walks): there are few
 // continuations (3 per env) and each is a long serial chain; a full warp of them leaves
-// fewer warps than the SMs have schedulers, 4-8 per warp multiply the warp instructions (measured sweep).  Blocks of WALK_WARPS warps.
+// fewer warps than the SMs have schedulers, 4-8 per warp multiply the warp instructions (measured sweep on the B200; on the H100 8 and 32 also lose to 16, DESIGN.md section 16).  Blocks of WALK_WARPS warps.
 // Expanded inside each continuation kernel (a macro, not an inlined function): the kernel's walk locals (the continuation, the view, the flags word)
 // are passed by address to the non-inlined stab_virtual, so they live in local memory, and behind an inlined function boundary the compiler lays
 // that frame out in another order — other stack offsets and registers in the stage that bounds a step.
