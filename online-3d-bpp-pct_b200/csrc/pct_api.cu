@@ -558,24 +558,24 @@ int pct_heuristic_actions_f64(pct_handle h, int32_t heuristic, double *d_rows, v
     return PCT_OK;
 }
 
+// The single queries are one row of one placement of the batched query kernels, asked and answered through the handle's scratch.
 int pct_query_placement_f64(pct_handle h, int32_t env, const double dims[3], double lx, double ly, double density, int32_t *feasible,
                             double *rest_height) {
     if (!h || !dims || !feasible || !rest_height || env < 0 || env >= h->n_envs) return PCT_ERR_INVALID;
     if (h->cfg.domain != PCT_CONTINUOUS) { h->err = "pct_query_placement_f64: continuous domain only (discrete: pct_query_placement)"; return PCT_ERR_INVALID; }
     if (!h->did_reset) { h->err = "pct_query_placement_f64 before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
-    if (!h->d_query_c) CK(h, cudaMalloc(&h->d_query_c, sizeof(double) * 2));
-    HParamsC hp{};
-    hp.code = PCT_H_QUERY_; hp.q_env = env; hp.q_den = density; hp.q_out = h->d_query_c;
-    hp.q[0] = dims[0]; hp.q[1] = dims[1]; hp.q[2] = dims[2]; hp.q[3] = lx; hp.q[4] = ly;
+    if (!h->d_query_c) CK(h, cudaMalloc(&h->d_query_c, sizeof(QueryOne<double>)));
+    QueryOne<double> *d = h->d_query_c;
+    QueryOne<double> one{density, {dims[0], dims[1], dims[2], lx, ly}, 0.0, env, 0};
     CK(h, cudaDeviceSynchronize());
-    CK(h, launch_heuristic_continuous(continuous_params(h), hp, h->own_stream));
+    CK(h, cudaMemcpyAsync(d, &one, sizeof one, cudaMemcpyHostToDevice, h->own_stream));
+    CK(h, launch_queries_continuous(continuous_params(h), QParams{&d->env, 1, 1, d->q, &d->density, &d->feasible, &d->rest}, h->own_stream));
     h->launches++;
-    double out[2];
-    CK(h, cudaMemcpyAsync(out, h->d_query_c, sizeof out, cudaMemcpyDeviceToHost, h->own_stream));
+    CK(h, cudaMemcpyAsync(&one, d, sizeof one, cudaMemcpyDeviceToHost, h->own_stream));
     CK(h, cudaStreamSynchronize(h->own_stream));
-    *feasible = out[0] != 0.0;
-    *rest_height = out[1];
+    *feasible = one.feasible;
+    *rest_height = one.rest;
     return PCT_OK;
 }
 
@@ -587,20 +587,29 @@ int pct_query_placement(pct_handle h, int32_t env, const int32_t dims[3], int32_
     CK(h, cudaSetDevice(h->device));
     const DParams p = discrete_params(h, 0, h->n_envs);
     if (p.W > HEUR_SIDE_MAX || p.L > HEUR_SIDE_MAX) { h->err = "pct_query_placement needs container sides <= 32"; return PCT_ERR_INVALID; }
-    const size_t cells = (size_t)p.W * p.L;
-    if (!h->d_query) CK(h, cudaMalloc(&h->d_query, sizeof(int32_t) * (2 + HEUR_SIDE_MAX * HEUR_SIDE_MAX)));
-    HParams hp{};
-    hp.code = PCT_H_QUERY_; hp.q_env = env; hp.q_den = density; hp.q_out = h->d_query;
-    hp.q[0] = dims[0]; hp.q[1] = dims[1]; hp.q[2] = dims[2]; hp.q[3] = lx; hp.q[4] = ly;
+    if (!h->d_query) CK(h, cudaMalloc(&h->d_query, sizeof(QueryOne<int32_t>) + sizeof(int32_t) * HEUR_SIDE_MAX * HEUR_SIDE_MAX));
+    QueryOne<int32_t> *d = h->d_query;
+    int32_t *d_map = (int32_t *)(d + 1);
+    QueryOne<int32_t> one{density, {dims[0], dims[1], dims[2], lx, ly}, 0, env, 0};
     CK(h, cudaDeviceSynchronize());
-    CK(h, launch_heuristic_discrete(p, hp, h->own_stream));
+    CK(h, cudaMemcpyAsync(d, &one, sizeof one, cudaMemcpyHostToDevice, h->own_stream));
+    CK(h, launch_queries_discrete(p, QParams{&d->env, 1, 1, d->q, &d->density, &d->feasible, &d->rest}, h->own_stream));
     h->launches++;
-    std::vector<int32_t> out(2 + cells);
-    CK(h, cudaMemcpyAsync(out.data(), h->d_query, sizeof(int32_t) * out.size(), cudaMemcpyDeviceToHost, h->own_stream));
+    if (height_map) {
+        CK(h, launch_height_maps(p, &d->env, 1, d_map, h->own_stream));
+        h->launches++;
+        CK(h, cudaMemcpyAsync(height_map, d_map, sizeof(int32_t) * p.W * p.L, cudaMemcpyDeviceToHost, h->own_stream));
+    }
+    CK(h, cudaMemcpyAsync(&one, d, sizeof one, cudaMemcpyDeviceToHost, h->own_stream));
     CK(h, cudaStreamSynchronize(h->own_stream));
-    *feasible = out[0];
-    *rest_height = out[1];
-    if (height_map) memcpy(height_map, out.data() + 2, sizeof(int32_t) * cells);
+    *feasible = one.feasible;
+    *rest_height = one.rest;
+    if (height_map)  // update_height_graph of a copy (returnMap, D:space.py:431): the footprint at its top, whatever the verdict
+        for (int i = 0; i < p.W; i++)
+            for (int j = 0; j < p.L; j++) {
+                const bool in = i >= lx && i < lx + dims[0] && j >= ly && j < ly + dims[1];
+                if (in) height_map[i * p.L + j] = one.rest + dims[2];
+            }
     return PCT_OK;
 }
 

@@ -17,6 +17,7 @@
 #include "pct_walks.cuh"
 #include "pct_continuous.cuh"
 #include "pct_cand_c.cuh"
+#include "pct_block.cuh"
 
 namespace pct {
 
@@ -579,7 +580,7 @@ __global__ void __launch_bounds__(64) pctc_feas_emit_kernel(const CParams p) {
     double (*rb)[5] = rb_store<PRE>();
     __shared__ uint32_t wb[2];
     __shared__ int lock;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, e = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31, e = blockIdx.x;
     CEnv *ev = p.env + e;
     const CHdr &h = ev->h;
     if (tid == 0) {
@@ -593,7 +594,7 @@ __global__ void __launch_bounds__(64) pctc_feas_emit_kernel(const CParams p) {
     GeomC g{ev->box, ev->den, n_box};
     EdgePool pool{ev->e_lower, ev->e_next, ev->e_off, ev->first_in, ev->last_in, ev->e_st, ev->e_st, h.n_edge,
                   ev->poly_off, &ev->poly[0][0], &ev->poly[0][0], h.n_poly};
-    int n_leaf = 0, fl = 0;
+    int fl = 0;
     if (PRE) {
         for (int t = tid; t < n_box; t += 64) {
             const double *b = ev->box[t];
@@ -602,40 +603,12 @@ __global__ void __launch_bounds__(64) pctc_feas_emit_kernel(const CParams p) {
         }
         __syncthreads();
     }
-#pragma unroll 1
-    for (int base = 0; base < n_cand && n_leaf < p.nl; base += 64) {
-        const int c = base + tid;
-        bool feas = false;
-        double t6[6] = {0, 0, 0, 0, 0, 0};
-        if (c < n_cand) {
-            cand_tuple(ev->cand[c], ev->ems, nb, t6);
-            // get_possible_position: x = xe - xs ... (C:bin3D.py:134-137); drop_box_virtual (C:space.py:380-425)
-            const double x = t6[3] - t6[0], y = t6[4] - t6[1], z = t6[5] - t6[2], lx = t6[0], ly = t6[1];
-            bool chk = !(lx + x - 1e-6 > p.W || ly + y - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
-            double mh = PRE ? rest_height_pre(rb, n_box, around6(-lx), around6(-ly), around6(lx + x), around6(ly + y))
-                            : rest_height_c(ev->box, 0, n_box, 1, lx, ly, lx + x, ly + y);
-            if (mh < 0) mh = 0.0;
-            if (mh + z - 1e-6 > p.H) chk = false;
-            if (!chk) feas = false;
-            else if (!STAB || fabs(mh) < 1e-6) feas = true;
-            else {
-                NodeC root{lx, ly, mh, x, y, z, x * y * z * den};
-                feas = stability_check<false, GeomC>(g, root, pool, &ev->big, &lock, 0, fl) != 0;
-            }
-        }
-        const uint32_t fm = __ballot_sync(FULL, feas);
-        if (lane == 0) wb[warp] = fm;
-        __syncthreads();
-        const int before = warp == 1 ? __popc(wb[0]) : 0, total = __popc(wb[0]) + __popc(wb[1]);
-        if (feas) {
-            const int k = n_leaf + before + __popc(fm & ((1u << lane) - 1));
-            if (k < p.nl)
-                for (int t = 0; t < 6; t++) leaf[k][t] = t6[t];
-        }
-        n_leaf += total;
-        __syncthreads();
-    }
-    if (n_leaf > p.nl) n_leaf = p.nl;
+    // get_possible_position: x = xe - xs ... (C:bin3D.py:134-137), the first `nl` feasible candidates in order
+    const int n_leaf = first_feasible<2>(n_cand, p.nl, leaf, wb, [&](int c, double *t6) {
+        cand_tuple(ev->cand[c], ev->ems, nb, t6);
+        double mh;
+        return place_virtual_c<STAB, PRE>(p, g, pool, &ev->big, &lock, t6[3] - t6[0], t6[4] - t6[1], t6[5] - t6[2], t6[0], t6[1], den, mh, fl, rb) != 0;
+    });
     fl = __reduce_or_sync(FULL, fl);
     if (fl && lane == 0) atomicOr(&ev->h.flags, fl);
     __syncthreads();

@@ -28,6 +28,7 @@
 #include "pct_geom.cuh"
 #include "pct_walks.cuh"
 #include "pct_obs.cuh"
+#include "pct_block.cuh"
 
 namespace pct {
 
@@ -669,122 +670,66 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K2_MINB) pct_candidates_
 #endif
 constexpr int FEAS_WARPS = FEAS_WARPS_N;
 constexpr int FEAS_THREADS = 32 * FEAS_WARPS;
-constexpr int K3_SMEM = sizeof(DEnvHot) + NL_MAX * 12 + 64 + EDGE_STAGE * 32 + POLY_STAGE * 16;
+// the block's shared memory: the staged env, the leaves in order, the rotation table of the item, the per-warp ballots of the compaction
+struct FeasSmD {
+    StageD s;
+    int16_t leaf[NL_MAX][6];
+    RotTab rt;
+    uint32_t wb[FEAS_WARPS];
+};
 
 template <typename OT, bool STAB, typename SlotT, bool DELTA = false>
 __global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(const DParams p) {
     constexpr int BITS = sizeof(SlotT) == 2 ? 4 : 8;
-    __shared__ __align__(16) unsigned char sm[K3_SMEM];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    __shared__ __align__(16) FeasSmD sm;
+    const int tid = threadIdx.x, lane = tid & 31;
     const int e = blockIdx.x;  // (round 1's heaviest-first permutation of this kernel went with the sorting pass; the legacy mode runs in env order)
-    DEnvHot *hot = (DEnvHot *)sm;
-    int16_t (*leaf)[6] = (int16_t (*)[6])(sm + sizeof(DEnvHot));
-    uint64_t *mbar = (uint64_t *)(sm + sizeof(DEnvHot) + NL_MAX * 12);
-    int *lock = (int *)(mbar + 1);
-    uint32_t *wb = (uint32_t *)(mbar + 2);             // per-warp feasibility ballots of the current pass
-    RotTab *rt = (RotTab *)(sm + sizeof(DEnvHot) + NL_MAX * 12 + 32);
-    Stack4 *st_sm = (Stack4 *)(sm + sizeof(DEnvHot) + NL_MAX * 12 + 64);
-    double *poly_sm = (double *)(st_sm + EDGE_STAGE);
+    DEnvHot *hot = &sm.s.hot;
     DEnvHot *ghot = p.hot + e;
     DEnvCold *cold = p.cold + e;
     KT_BEGIN();
-    if (tid == 0) {
-        *lock = 0;
-        mbar_init(mbar, 1);
-        fence_proxy_async();
-    }
-    __syncthreads();
-    if (tid == 0) {
-        if (p.ready) {  // overlapped mode: wait for the candidates kernel's hand-over of THIS env
-            if (!env_wait(p.ready + p.n_envs + e, p.epoch)) atomicOr(&ghot->h.flags, PCT_FLAG_SYNC_TIMEOUT);
-            fence_proxy_async_all();
-        }
-        mbar_expect_tx(mbar, (uint32_t)sizeof(DEnvHot));
-        tma_load_1d(hot, ghot, (uint32_t)sizeof(DEnvHot), mbar);
-    }
-    mbar_wait(mbar, 0);
-    __syncthreads();  // every thread must have observed phase 0 before the barrier is re-armed
+    StagedD sd = stage_env_d<STAB>(sm.s, p, e, true);
     const DHdr &h = hot->h;
-    if (STAB && h.n_edge > 0) {  // stage the load edges (second phase of the same mbarrier)
-        const uint32_t bytes = (uint32_t)min(h.n_edge, EDGE_STAGE) * (uint32_t)sizeof(Stack4);
-        const uint32_t pbytes = (uint32_t)min(h.n_poly, POLY_STAGE) * 16u;
-        if (tid == 0) {
-            mbar_expect_tx(mbar, bytes + pbytes);
-            tma_load_1d(st_sm, cold->e_st, bytes, mbar);
-            if (pbytes) tma_load_1d(poly_sm, cold->poly, pbytes, mbar);
-        }
-        mbar_wait(mbar, 1);
-    }
     const int nb3[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
-    if (tid == 0) make_rot_tab(nb3, p.setting == 2 ? 6 : 2, *rt);
+    if (tid == 0) make_rot_tab(nb3, p.setting == 2 ? 6 : 2, sm.rt);
     __syncthreads();
-    const int n_cand = h.n_cand, n_box = h.n_box;
+    const int n_cand = h.n_cand;
     const double den = h.next_den;
     const SlotT *cand = (const SlotT *)cold->cand;
-    GeomD g{hot->box, n_box, p.setting == 3 ? cold->density : nullptr};
-    EdgePool pool{hot->e_lower, hot->e_next, hot->e_off, hot->first_in, hot->last_in, cold->e_st, st_sm, h.n_edge,
-                  hot->poly_off, &cold->poly[0][0], poly_sm, h.n_poly};
-    int n_leaf = 0, fl = 0;
+    const RotTab *rt = &sm.rt;
+    int fl = 0;
     // ---------------- get_possible_position (D:bin3D.py:100-136): first `nl` feasible candidates in order ----------------
-#pragma unroll 1
-    for (int base = 0; base < n_cand && n_leaf < p.nl; base += FEAS_THREADS) {
-        const int c = base + tid;
-        bool feas = false;
-        int xs = 0, ys = 0, zs = 0, rot = 0, sx = 0, sy = 0, sz = 0;
-        if (c < n_cand) {
-            key_unpack<BITS>(cand[c], xs, ys, zs, rot);
-            sx = rt->d[rot][0]; sy = rt->d[rot][1]; sz = rt->d[rot][2];
-            // drop_box_virtual (D:space.py:393-433) + check_box (:436-454)
-            const int mh = rest_height(hot->box, 0, n_box, 1, xs, ys, xs + sx, ys + sy);
-            if (xs + sx > p.W || ys + sy > p.L) feas = false;
-            else if (mh + sz > p.H) feas = false;
-            else if (!STAB || mh == 0) feas = true;
-            else {
-                NodeD root{xs, ys, mh, sx, sy, sz, (double)(sx * sy * sz) * den};
+    const int n_leaf = first_feasible<FEAS_WARPS>(n_cand, p.nl, sm.leaf, sm.wb, [&](int c, int16_t *row) {
+        int xs, ys, zs, rot, mh;
+        key_unpack<BITS>(cand[c], xs, ys, zs, rot);
+        const int sx = rt->d[rot][0], sy = rt->d[rot][1], sz = rt->d[rot][2];
 #ifdef PCT_PHASE_TIMERS
-                const long long c0 = clock64();
-                int fl2 = 0;
-                long long prof[6];
-                feas = stability_check<false, GeomD>(g, root, pool, &cold->big, lock, 0, fl2, prof) != 0;
-                const long long dc = clock64() - c0;
-                fl |= fl2 & 0xFFFF;
-                if (p.mode == 1 && p.dbg) {
-                    unsigned long long packed = ((unsigned long long)dc << 24) | ((unsigned long long)((fl2 >> 16) & 0xFF) << 8) | (unsigned long long)((fl2 >> 24) & 0xFF);
-                    long long *slot = &p.dbg[(size_t)(p.env_id_base + e - p.env_id_base0) * 16];
-                    if (atomicMax((unsigned long long *)&slot[12], packed) < packed)
-                        { slot[3] = prof[0]; slot[7] = prof[1]; slot[11] = prof[2]; slot[13] = prof[3]; slot[14] = prof[4]; }
-                }
+        const long long c0 = clock64();
+        int fl2 = 0;
+        long long prof[6];
+        const bool feas = place_virtual_d<STAB>(p, sd.g, sd.pool, &cold->big, &sm.s.lock, sx, sy, sz, xs, ys, den, mh, fl2, prof) != 0;
+        const long long dc = clock64() - c0;
+        fl |= fl2 & 0xFFFF;
+        // recorded only for placements that ran the stability check (it counts its visits from bit 16 of fl2); dc also covers the
+        // resting height and the bounds tests in front of it
+        if (p.mode == 1 && p.dbg && (fl2 >> 16) != 0) {
+            unsigned long long packed = ((unsigned long long)dc << 24) | ((unsigned long long)((fl2 >> 16) & 0xFF) << 8) | (unsigned long long)((fl2 >> 24) & 0xFF);
+            long long *slot = &p.dbg[(size_t)(p.env_id_base + e - p.env_id_base0) * 16];
+            if (atomicMax((unsigned long long *)&slot[12], packed) < packed)
+                { slot[3] = prof[0]; slot[7] = prof[1]; slot[11] = prof[2]; slot[13] = prof[3]; slot[14] = prof[4]; }
+        }
 #else
-                feas = stability_check<false, GeomD>(g, root, pool, &cold->big, lock, 0, fl) != 0;
+        const bool feas = place_virtual_d<STAB>(p, sd.g, sd.pool, &cold->big, &sm.s.lock, sx, sy, sz, xs, ys, den, mh, fl) != 0;
 #endif
-            }
-        }
-        const uint32_t fm = __ballot_sync(FULL, feas);
-        if (lane == 0) wb[warp] = fm;
-        __syncthreads();
-        int before = 0, total = 0;
-#pragma unroll
-        for (int w = 0; w < FEAS_WARPS; w++) {
-            const int cnt = __popc(wb[w]);
-            if (w < warp) before += cnt;
-            total += cnt;
-        }
-        if (feas) {
-            const int k = n_leaf + before + __popc(fm & ((1u << lane) - 1));
-            if (k < p.nl) {
-                leaf[k][0] = (int16_t)xs; leaf[k][1] = (int16_t)ys; leaf[k][2] = (int16_t)zs;
-                leaf[k][3] = (int16_t)(xs + sx); leaf[k][4] = (int16_t)(ys + sy); leaf[k][5] = (int16_t)(zs + sz);
-            }
-        }
-        n_leaf += total;
-        __syncthreads();
-    }
-    if (n_leaf > p.nl) n_leaf = p.nl;
+        row[0] = (int16_t)xs; row[1] = (int16_t)ys; row[2] = (int16_t)zs;
+        row[3] = (int16_t)(xs + sx); row[4] = (int16_t)(ys + sy); row[5] = (int16_t)(zs + sz);
+        return feas;
+    });
     fl = __reduce_or_sync(FULL, fl);
     if (fl && lane == 0) atomicOr(&ghot->h.flags, fl);
     __syncthreads();
     // persist the emitted leaves for the leaf-index action path; header / info
-    for (int t = tid; t < n_leaf * 6; t += FEAS_THREADS) ((int16_t *)cold->leaf)[t] = ((int16_t *)leaf)[t];
+    for (int t = tid; t < n_leaf * 6; t += FEAS_THREADS) ((int16_t *)cold->leaf)[t] = ((int16_t *)sm.leaf)[t];
     if (tid == 0) {
         ghot->h.n_leaf = n_leaf;
         if (p.info) {
@@ -795,8 +740,8 @@ __global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(co
         }
     }
     // ---------------- cur_observation (D:bin3D.py:70-93) ----------------
-    if constexpr (DELTA) write_obs_delta<OT>(p, e, hot, cold, leaf, n_leaf, tid, FEAS_THREADS);
-    else write_obs<OT>(p, e, hot, cold, leaf, n_leaf, tid, FEAS_THREADS);
+    if constexpr (DELTA) write_obs_delta<OT>(p, e, hot, cold, sm.leaf, n_leaf, tid, FEAS_THREADS);
+    else write_obs<OT>(p, e, hot, cold, sm.leaf, n_leaf, tid, FEAS_THREADS);
     if (tid == 0) KT_END(p.env_id_base + e - p.env_id_base0, 2);
 }
 

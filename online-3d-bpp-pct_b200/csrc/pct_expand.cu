@@ -4,8 +4,8 @@
 // One block of EXPAND_THREADS per row, which takes the row's k items in turn.  Per item:
 //   warp 0    the ordered candidate list with the candidates kernel's own routines (build_candidates and the EV / EP / CP / FC generators,
 //             pct_cand.cuh; PCTC_CANDIDATES_BODY, pct_cand_c.cuh), then the keyed shuffle, into the env's candidate scratch;
-//   block     one thread per candidate in EXPAND_THREADS chunks: bounds, resting height and stability_check<false>, the code of the step's
-//             block-mode feasibility kernel; ordered compaction of the first `nl` feasible candidates;
+//   block     one thread per candidate in EXPAND_THREADS chunks: the placement test and the ordered compaction of the first `nl` feasible
+//             candidates of the step's block-mode feasibility kernel (place_virtual_d / _c and first_feasible, pct_block.cuh);
 //   out       the leaf rows as the observation carries them, and the info record pct_set_items would write.
 // The pooled walk stage is not used: its pools and counters belong to the step.
 //
@@ -21,24 +21,22 @@
 #include "pct_geom_continuous.cuh"
 #include "pct_continuous.cuh"
 #include "pct_cand_c.cuh"
+#include "pct_block.cuh"
 
 namespace pct {
 
-constexpr int EXPAND_THREADS = 64;  // two warps: the compaction below adds up the ballots of warps 0 and 1
+constexpr int EXPAND_THREADS = 64;
 
-// shared memory of one discrete block: the staged record (TMA), the set emulation's tables (the 2048-slot stage included), the leaves
+// shared memory of one discrete block: the staged env, the set emulation's tables (the 2048-slot stage included), the leaves
 template <typename SlotT>
 struct ExpandSmD {
-    DEnvHot hot;
+    StageD s;
     SlotT tabA[TAB_A], tabB[TAB_B];
     SetStage stg;
     int16_t leaf[NL_MAX][6];
-    alignas(16) Stack4 st[EDGE_STAGE];
-    alignas(16) double poly[POLY_STAGE * 2];
-    uint64_t mbar;
     RotTab rt;
-    int lock, fl, n_cand;
-    uint32_t wb[2];
+    int fl, n_cand;
+    uint32_t wb[EXPAND_THREADS / 32];
 };
 
 // zero rows and a zero record for a row whose env index is outside the handle
@@ -58,36 +56,11 @@ __global__ void __launch_bounds__(EXPAND_THREADS) pct_expand_kernel(const DParam
     const int e = x.env ? x.env[r] : r;
     const size_t row = (size_t)r * K;
     if (e < 0 || e >= p.n_envs) { expand_zero_row<OT>(x, nl, row, tid); return; }
-    DEnvHot *hot = &s.hot;
+    const DEnvHot *hot = &s.s.hot;
     DEnvCold *cold = p.cold + e;
-    if (tid == 0) {
-        s.lock = 0;
-        mbar_init(&s.mbar, 1);
-        fence_proxy_async();
-    }
-    __syncthreads();
-    if (tid == 0) {
-        mbar_expect_tx(&s.mbar, (uint32_t)sizeof(DEnvHot));
-        tma_load_1d(hot, p.hot + e, (uint32_t)sizeof(DEnvHot), &s.mbar);
-    }
-    mbar_wait(&s.mbar, 0);
-    __syncthreads();
+    StagedD sd = stage_env_d<STAB>(s.s, p, e, false);
     const DHdr &h = hot->h;
-    if (STAB && h.n_edge > 0) {  // the first load edges and polygon vertices (second phase of the same mbarrier)
-        const uint32_t bytes = (uint32_t)min(h.n_edge, EDGE_STAGE) * (uint32_t)sizeof(Stack4);
-        const uint32_t pbytes = (uint32_t)min(h.n_poly, POLY_STAGE) * 16u;
-        if (tid == 0) {
-            mbar_expect_tx(&s.mbar, bytes + pbytes);
-            tma_load_1d(s.st, cold->e_st, bytes, &s.mbar);
-            if (pbytes) tma_load_1d(s.poly, cold->poly, pbytes, &s.mbar);
-        }
-        mbar_wait(&s.mbar, 1);
-    }
-    __syncthreads();
     const int n_box = h.n_box, R = p.setting == 2 ? 6 : 2;
-    GeomD g{hot->box, n_box, p.setting == 3 ? cold->density : nullptr};
-    EdgePool pool{hot->e_lower, hot->e_next, hot->e_off, hot->first_in, hot->last_in, cold->e_st, s.st, h.n_edge,
-                  hot->poly_off, &cold->poly[0][0], s.poly, h.n_poly};
     SlotT *const out = (SlotT *)cold->cand;
     const RotTab *rt = &s.rt;
 #pragma unroll 1
@@ -131,39 +104,16 @@ __global__ void __launch_bounds__(EXPAND_THREADS) pct_expand_kernel(const DParam
         __syncthreads();
         // ---- get_possible_position: first `nl` feasible candidates in order (the step's block-mode feasibility kernel) ----
         const int n_cand = s.n_cand;
-        int n_leaf = 0, fl = 0;
-#pragma unroll 1
-        for (int base = 0; base < n_cand && n_leaf < nl; base += EXPAND_THREADS) {
-            const int c = base + tid;
-            bool feas = false;
-            int xs = 0, ys = 0, zs = 0, rot = 0, sx = 0, sy = 0, sz = 0;
-            if (c < n_cand) {
-                key_unpack<KB>(out[c], xs, ys, zs, rot);
-                sx = rt->d[rot][0]; sy = rt->d[rot][1]; sz = rt->d[rot][2];
-                const int mh = rest_height(hot->box, 0, n_box, 1, xs, ys, xs + sx, ys + sy);
-                if (xs + sx > p.W || ys + sy > p.L) feas = false;
-                else if (mh + sz > p.H) feas = false;
-                else if (!STAB || mh == 0) feas = true;
-                else {
-                    NodeD root{xs, ys, mh, sx, sy, sz, (double)(sx * sy * sz) * den};
-                    feas = stability_check<false, GeomD>(g, root, pool, &cold->big, &s.lock, 0, fl) != 0;
-                }
-            }
-            const uint32_t fm = __ballot_sync(FULL, feas);
-            if (lane == 0) s.wb[warp] = fm;
-            __syncthreads();
-            const int before = warp == 1 ? __popc(s.wb[0]) : 0, total = __popc(s.wb[0]) + __popc(s.wb[1]);
-            if (feas) {
-                const int kk = n_leaf + before + __popc(fm & ((1u << lane) - 1));
-                if (kk < nl) {
-                    s.leaf[kk][0] = (int16_t)xs; s.leaf[kk][1] = (int16_t)ys; s.leaf[kk][2] = (int16_t)zs;
-                    s.leaf[kk][3] = (int16_t)(xs + sx); s.leaf[kk][4] = (int16_t)(ys + sy); s.leaf[kk][5] = (int16_t)(zs + sz);
-                }
-            }
-            n_leaf += total;
-            __syncthreads();
-        }
-        if (n_leaf > nl) n_leaf = nl;
+        int fl = 0;
+        const int n_leaf = first_feasible<EXPAND_THREADS / 32>(n_cand, nl, s.leaf, s.wb, [&](int c, int16_t *row) {
+            int xs, ys, zs, rot, mh;
+            key_unpack<KB>(out[c], xs, ys, zs, rot);
+            const int sx = rt->d[rot][0], sy = rt->d[rot][1], sz = rt->d[rot][2];
+            const bool feas = place_virtual_d<STAB>(p, sd.g, sd.pool, &cold->big, &s.s.lock, sx, sy, sz, xs, ys, den, mh, fl) != 0;
+            row[0] = (int16_t)xs; row[1] = (int16_t)ys; row[2] = (int16_t)zs;
+            row[3] = (int16_t)(xs + sx); row[4] = (int16_t)(ys + sy); row[5] = (int16_t)(zs + sz);
+            return feas;
+        });
         fl = __reduce_or_sync(FULL, fl);
         if (fl && lane == 0) atomicOr(&s.fl, fl);
         __syncthreads();
@@ -198,7 +148,7 @@ __global__ void __launch_bounds__(EXPAND_THREADS) pctc_expand_kernel(const CPara
     __shared__ uint32_t rs_c[32];
     __shared__ uint16_t stg_c[32];
     __shared__ double leaf[NL_MAX][6];
-    __shared__ uint32_t wb[2];
+    __shared__ uint32_t wb[EXPAND_THREADS / 32];
     __shared__ int lock, s_fl, s_cnt;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, r = blockIdx.x, K = x.k, nl = p.nl;
     const int e = x.env ? x.env[r] : r;
@@ -224,39 +174,12 @@ __global__ void __launch_bounds__(EXPAND_THREADS) pctc_expand_kernel(const CPara
         __syncthreads();
         // ---- get_possible_position (the step's block-mode feasibility kernel, pctc_feas_emit_kernel) ----
         const int n_cand = s_cnt;
-        int n_leaf = 0, fl = 0;
-#pragma unroll 1
-        for (int base = 0; base < n_cand && n_leaf < nl; base += EXPAND_THREADS) {
-            const int c = base + tid;
-            bool feas = false;
-            double t6[6] = {0, 0, 0, 0, 0, 0};
-            if (c < n_cand) {
-                cand_tuple(ev->cand[c], ev->ems, nb, t6);
-                const double x6 = t6[3] - t6[0], y6 = t6[4] - t6[1], z6 = t6[5] - t6[2], lx = t6[0], ly = t6[1];
-                bool chk = !(lx + x6 - 1e-6 > p.W || ly + y6 - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
-                double mh = rest_height_c(ev->box, 0, n_box, 1, lx, ly, lx + x6, ly + y6);
-                if (mh < 0) mh = 0.0;
-                if (mh + z6 - 1e-6 > p.H) chk = false;
-                if (!chk) feas = false;
-                else if (!STAB || fabs(mh) < 1e-6) feas = true;
-                else {
-                    NodeC root{lx, ly, mh, x6, y6, z6, x6 * y6 * z6 * den};
-                    feas = stability_check<false, GeomC>(g, root, pool, &ev->big, &lock, 0, fl) != 0;
-                }
-            }
-            const uint32_t fm = __ballot_sync(FULL, feas);
-            if (lane == 0) wb[warp] = fm;
-            __syncthreads();
-            const int before = warp == 1 ? __popc(wb[0]) : 0, total = __popc(wb[0]) + __popc(wb[1]);
-            if (feas) {
-                const int kk = n_leaf + before + __popc(fm & ((1u << lane) - 1));
-                if (kk < nl)
-                    for (int t = 0; t < 6; t++) leaf[kk][t] = t6[t];
-            }
-            n_leaf += total;
-            __syncthreads();
-        }
-        if (n_leaf > nl) n_leaf = nl;
+        int fl = 0;
+        const int n_leaf = first_feasible<EXPAND_THREADS / 32>(n_cand, nl, leaf, wb, [&](int c, double *t6) {
+            cand_tuple(ev->cand[c], ev->ems, nb, t6);
+            double mh;
+            return place_virtual_c<STAB>(p, g, pool, &ev->big, &lock, t6[3] - t6[0], t6[4] - t6[1], t6[5] - t6[2], t6[0], t6[1], den, mh, fl) != 0;
+        });
         fl = __reduce_or_sync(FULL, fl);
         if (fl && lane == 0) atomicOr(&s_fl, fl);
         __syncthreads();

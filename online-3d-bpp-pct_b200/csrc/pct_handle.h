@@ -4,6 +4,19 @@
 #include <vector>
 #include "pct_kernels.h"
 
+namespace pct {
+// One row of the batched query kernels with its answer (n = k = 1): the scratch of the single-placement queries.  The discrete one is
+// followed by a W x L height map.
+template <typename T>
+struct QueryOne {
+    double density;
+    T q[5];                  // oriented dims, lx, ly
+    T rest;
+    int32_t env;
+    uint8_t feasible;
+};
+}  // namespace pct
+
 struct pct_env_batch {
     pct_config cfg;
     int n_envs = 0, device = 0;
@@ -43,8 +56,8 @@ struct pct_env_batch {
     int32_t *d_hstate = nullptr;  // (n_envs, 4) LSAH footprint state (pct_heuristic_actions; discrete handles)
     double *d_hstate_c = nullptr; // same for the continuous domain (pct_heuristic_actions_f64)
     uint64_t snap_fp = 0;         // fingerprint written into / required of snapshot records (pct_snapshot.cu)
-    double *d_query_c = nullptr;  // 2 doubles: result of pct_query_placement_f64
-    int32_t *d_query = nullptr;   // 2 + W*L ints: result of pct_query_placement
+    pct::QueryOne<double> *d_query_c = nullptr;  // pct_query_placement_f64
+    pct::QueryOne<int32_t> *d_query = nullptr;   // pct_query_placement, then HEUR_SIDE_MAX^2 ints for the height map
     int item_mode = 0;
     // staging for the host-buffer entry points
     void *d_obs = nullptr, *d_act = nullptr;

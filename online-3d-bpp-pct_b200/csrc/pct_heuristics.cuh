@@ -2,19 +2,19 @@
 //
 // Every baseline of the reference is the same loop: enumerate placements in a fixed order, ask
 // Space.drop_box_virtual for feasibility (+ the rest height / the updated height map), score, keep the best under a strict
-// comparison.  Here a block of 64 threads owns one env (staged in shared memory exactly like pct_feas_emit_kernel), every
-// thread evaluates one placement of the current 64-chunk with the same feasibility code the leaf expansion uses, and
+// comparison.  Here a block of 64 threads owns one env (staged in shared memory by stage_env_d, pct_block.cuh), every
+// thread evaluates one placement of the current 64-chunk with the placement test of the leaf expansion (place_virtual_d), and
 // thread 0 folds the chunk's verdicts in enumeration order, so ties resolve exactly as in the sequential reference.
 // The result is an ACTION ROW per env ([lx, ly, 0, lx+x, ly+y, 0, 0, 0, 1] — what LeafNode2Action decodes back into the
 // chosen orientation), fed to the ordinary pct_step.  "No feasible placement" (the baselines then end the episode without
 // stepping) is encoded as a row no item can match, which makes pct_step end the episode with the same counter / ratio.
 //
-// Included at the end of pct_discrete.cu (same translation unit: it reuses GeomD / rest_height / the staging layout).
+// Included at the end of pct_discrete.cu (same translation unit: it reuses FEAS_THREADS and rest_height).
 #pragma once
 
 namespace pct {
 
-constexpr int HM_CELLS_MAX = 1024;   // height map staged in shared memory (HM, MACS, placement queries): W * L <= 1024
+constexpr int HM_CELLS_MAX = 1024;   // height map staged in shared memory (HM, MACS): W * L <= 1024
 constexpr int HC_MAX = 6144;         // RANDOM: feasibility bitmap capacity (grid x rotations)
 
 // Large-container instantiation (BIG = true: HM, MACS and RANDOM when W or L > 32).  The height map, the RANDOM bitmap and MACS's
@@ -42,30 +42,6 @@ __device__ __forceinline__ void heur_rot(const int nb[3], int rot, int &x, int &
 }
 
 struct HCand { int sx, sy, sz, lx, ly, ex, ey, ez; bool valid; };
-
-// Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) + check_box (D:space.py:393-454) of ONE placement
-// of a staged env, for the batched queries (pct_query.cuh).  It is the PCT_H_QUERY_ branch below, expression for expression (same
-// rest_height, same stability_check instantiation).  That branch keeps its own inline copy because routing it through this function
-// changes the register allocation of pct_heuristic_kernel; tests/test_gpu_queries.py pins the two paths to each other.  A position
-// outside [0, W) x [0, L) or a zero footprint is infeasible with rest height 0; a footprint that sticks out of the container is
-// infeasible with its rest height reported.  Raised capacity flags go to `fl` (the callers do not OR them into the env).
-template <bool STAB>
-__device__ __forceinline__ int query_placement_d(const DEnvHot *hot, int n_box, const GeomD &g, EdgePool &pool, BigScratch *big, int *lock,
-                                                 int W, int L, int H, int sx, int sy, int sz, int lx, int ly, double den, int &mh, int &fl) {
-    int feas = 0;
-    mh = 0;
-    if (lx >= 0 && ly >= 0 && lx < W && ly < L && sx > 0 && sy > 0) {
-        mh = rest_height(hot->box, 0, n_box, 1, lx, ly, lx + sx, ly + sy);
-        if (lx + sx > W || ly + sy > L) feas = 0;
-        else if (mh + sz > H) feas = 0;
-        else if (!STAB || mh == 0) feas = 1;
-        else {
-            NodeD root{lx, ly, mh, sx, sy, sz, (double)(sx * sy * sz) * den};
-            feas = stability_check<false, GeomD>(g, root, pool, big, lock, 0, fl) != 0;
-        }
-    }
-    return feas;
-}
 
 // enumeration index -> placement.  EMS family: ems (list order; OnlineBPH: deep-bottom-left order) x rot [x corner];
 // grid family: lx x ly x rot with the loop bounds of the UNROTATED item (heuristic.py:253-254).
@@ -129,10 +105,10 @@ __device__ __noinline__ long long macs_score(const int16_t *hm, int W, int L, co
 // BIG (see heur_big_smem): launched with the dynamic shared memory of the container, for HM / MACS / RANDOM only.
 template <bool STAB, bool BIG>
 __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DParams p, const HParams hp) {
-    __shared__ __align__(16) unsigned char sm[K3_SMEM];
+    __shared__ __align__(16) StageD sm;
     __shared__ int16_t hm_s[BIG ? 1 : HM_CELLS_MAX];
     __shared__ uint8_t ord[E_MAX];
-    __shared__ int c_feas[FEAS_THREADS], c_mh[FEAS_THREADS];
+    __shared__ int c_feas[FEAS_THREADS];
     __shared__ long long c_score[FEAS_THREADS];
     __shared__ uint32_t fbits_s[BIG ? 1 : HC_MAX / 32];
     __shared__ int hm_sum, stop;
@@ -140,45 +116,20 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
     int16_t *const hm = BIG ? (int16_t *)heur_dyn : hm_s;
     uint32_t *const fbits = BIG ? (uint32_t *)(heur_dyn + heur_big_map_bytes(p.W, p.L)) : fbits_s;
     const int tid = threadIdx.x, lane = tid & 31;
-    const int code = hp.code;
-    const int e = code == PCT_H_QUERY_ ? hp.q_env : blockIdx.x;
-    DEnvHot *hot = (DEnvHot *)sm;
-    uint64_t *mbar = (uint64_t *)(sm + sizeof(DEnvHot) + NL_MAX * 12);
-    int *lock = (int *)(mbar + 1);
-    Stack4 *st_sm = (Stack4 *)(sm + sizeof(DEnvHot) + NL_MAX * 12 + 64);
-    double *poly_sm = (double *)(st_sm + EDGE_STAGE);
+    const int code = hp.code, e = blockIdx.x;
+    const DEnvHot *hot = &sm.hot;
     DEnvHot *ghot = p.hot + e;
-    DEnvCold *cold = p.cold + e;
     if (tid == 0) {
-        *lock = 0;
         hm_sum = 0;
         stop = 0;
-        mbar_init(mbar, 1);
-        fence_proxy_async();
     }
-    __syncthreads();
-    if (tid == 0) {
-        mbar_expect_tx(mbar, (uint32_t)sizeof(DEnvHot));
-        tma_load_1d(hot, ghot, (uint32_t)sizeof(DEnvHot), mbar);
-    }
-    mbar_wait(mbar, 0);
-    __syncthreads();
+    StagedD sd = stage_env_d<STAB>(sm, p, e, false);
     const DHdr &h = hot->h;
-    if (STAB && h.n_edge > 0) {
-        const uint32_t bytes = (uint32_t)min(h.n_edge, EDGE_STAGE) * (uint32_t)sizeof(Stack4);
-        const uint32_t pbytes = (uint32_t)min(h.n_poly, POLY_STAGE) * 16u;
-        if (tid == 0) {
-            mbar_expect_tx(mbar, bytes + pbytes);
-            tma_load_1d(st_sm, cold->e_st, bytes, mbar);
-            if (pbytes) tma_load_1d(poly_sm, cold->poly, pbytes, mbar);
-        }
-        mbar_wait(mbar, 1);
-    }
     const int W = p.W, L = p.L, n_box = h.n_box, n_ems = h.n_ems;
     const int nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
     const int R = p.setting == 2 ? 6 : 2;
-    const double den = code == PCT_H_QUERY_ ? hp.q_den : h.next_den;
-    const bool need_map = code == PCT_H_HM || code == PCT_H_MACS || code == PCT_H_QUERY_;
+    const double den = h.next_den;
+    const bool need_map = code == PCT_H_HM || code == PCT_H_MACS;
     if (need_map) {  // Space.plain (D:space.py:316-326): per cell the highest top among the boxes covering it
         int part = 0;
         for (int c = tid; c < W * L; c += FEAS_THREADS) {
@@ -202,39 +153,7 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
         }
     }
     __syncthreads();
-    GeomD g{hot->box, n_box, p.setting == 3 ? cold->density : nullptr};
-    EdgePool pool{hot->e_lower, hot->e_next, hot->e_off, hot->first_in, hot->last_in, cold->e_st, st_sm, h.n_edge,
-                  hot->poly_off, &cold->poly[0][0], poly_sm, h.n_poly};
     int fl = 0;
-
-    if (code == PCT_H_QUERY_) {
-        HCand k{hp.q[0], hp.q[1], hp.q[2], hp.q[3], hp.q[4], 0, 0, 0, true};
-        int feas = 0, mh = 0;
-        if (tid == 0) {
-            if (k.lx >= 0 && k.ly >= 0 && k.lx < W && k.ly < L && k.sx > 0 && k.sy > 0) {
-                mh = rest_height(hot->box, 0, n_box, 1, k.lx, k.ly, k.lx + k.sx, k.ly + k.sy);
-                if (k.lx + k.sx > W || k.ly + k.sy > L) feas = 0;
-                else if (mh + k.sz > p.H) feas = 0;
-                else if (!STAB || mh == 0) feas = 1;
-                else {
-                    NodeD root{k.lx, k.ly, mh, k.sx, k.sy, k.sz, (double)(k.sx * k.sy * k.sz) * den};
-                    feas = stability_check<false, GeomD>(g, root, pool, &cold->big, lock, 0, fl) != 0;
-                }
-            }
-            hp.q_out[0] = feas;
-            hp.q_out[1] = mh;
-            c_mh[0] = mh;
-        }
-        __syncthreads();
-        mh = c_mh[0];
-        for (int c = tid; c < W * L; c += FEAS_THREADS) {  // update_height_graph of a copy (returnMap, D:space.py:431)
-            const int i = c / L, j = c - i * L;
-            const bool in = i >= k.lx && i < k.lx + k.sx && j >= k.ly && j < k.ly + k.sy;
-            hp.q_out[2 + c] = in ? mh + k.sz : (int)hm[c];
-        }
-        return;
-    }
-
     int ny = 1, n_c;
     if (code <= PCT_H_MACS) n_c = n_ems * R * (code == PCT_H_MACS ? 4 : 1);
     else {
@@ -267,17 +186,7 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
         long long score = 0;
         if (c < n_c) {
             const HCand k = heur_decode(code, c, hot->ems, ord, nb, R, ny);
-            if (k.valid) {
-                // Space.drop_box_virtual + check_box (D:space.py:393-454)
-                mh = rest_height(hot->box, 0, n_box, 1, k.lx, k.ly, k.lx + k.sx, k.ly + k.sy);
-                if (k.lx + k.sx > W || k.ly + k.sy > L) feas = 0;
-                else if (mh + k.sz > p.H) feas = 0;
-                else if (!STAB || mh == 0) feas = 1;
-                else {
-                    NodeD root{k.lx, k.ly, mh, k.sx, k.sy, k.sz, (double)(k.sx * k.sy * k.sz) * den};
-                    feas = stability_check<false, GeomD>(g, root, pool, &cold->big, lock, 0, fl) != 0;
-                }
-            }
+            if (k.valid) feas = place_virtual_d<STAB>(p, sd.g, sd.pool, &p.cold[e].big, &sm.lock, k.sx, k.sy, k.sz, k.lx, k.ly, den, mh, fl);
             if (feas) {
                 const int top = mh + k.sz;
                 if (code == PCT_H_LSAH) {  // heuristic.py:196-200
@@ -303,7 +212,6 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
             }
         }
         c_feas[tid] = feas;
-        c_mh[tid] = mh;
         c_score[tid] = score;
         if (code == PCT_H_RANDOM && feas) atomicOr(&fbits[c >> 5], 1u << (c & 31));
         __syncthreads();
@@ -365,13 +273,12 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_heuristic_kernel(const DP
 }
 
 cudaError_t launch_heuristic_discrete(const DParams &p, const HParams &hp, cudaStream_t st) {
-    const int grid = hp.code == PCT_H_QUERY_ ? 1 : p.n_envs;
     if ((p.W > HEUR_SIDE_MAX || p.L > HEUR_SIDE_MAX) && (hp.code == PCT_H_HM || hp.code == PCT_H_MACS || hp.code == PCT_H_RANDOM)) {
         const size_t smem = heur_big_smem(p.W, p.L, p.setting == 2 ? 6 : 2);
-        if (p.setting == 2) pct_heuristic_kernel<false, true><<<grid, FEAS_THREADS, smem, st>>>(p, hp);
-        else pct_heuristic_kernel<true, true><<<grid, FEAS_THREADS, smem, st>>>(p, hp);
-    } else if (p.setting == 2) pct_heuristic_kernel<false, false><<<grid, FEAS_THREADS, 0, st>>>(p, hp);
-    else pct_heuristic_kernel<true, false><<<grid, FEAS_THREADS, 0, st>>>(p, hp);
+        if (p.setting == 2) pct_heuristic_kernel<false, true><<<p.n_envs, FEAS_THREADS, smem, st>>>(p, hp);
+        else pct_heuristic_kernel<true, true><<<p.n_envs, FEAS_THREADS, smem, st>>>(p, hp);
+    } else if (p.setting == 2) pct_heuristic_kernel<false, false><<<p.n_envs, FEAS_THREADS, 0, st>>>(p, hp);
+    else pct_heuristic_kernel<true, false><<<p.n_envs, FEAS_THREADS, 0, st>>>(p, hp);
     return cudaGetLastError();
 }
 

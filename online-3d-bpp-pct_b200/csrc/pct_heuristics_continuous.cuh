@@ -2,8 +2,8 @@
 // (tools.py:217-218; heuristic.py LASH :138-226, OnlineBPH :364-424, BR :500-577 over pct_envs.PctContinuous0).
 //
 // Same scheme as pct_heuristics.cuh: a block of 64 threads owns one env, every thread evaluates one (EMS, orientation)
-// placement of the current 64-chunk with the feasibility code of the leaf expansion (pctc_feas_emit_kernel: bounds with the
-// 1e-6 tolerances, interSect2D rest height, virtual stability), and thread 0 folds the chunk in enumeration order so that
+// placement of the current 64-chunk with the placement test of the leaf expansion (place_virtual_c, pct_block.cuh: bounds with
+// the 1e-6 tolerances, interSect2D rest height, virtual stability), and thread 0 folds the chunk in enumeration order so that
 // ties resolve as in the sequential reference.  All scores are float64 and written with the reference's operand order
 // (the translation unit is compiled with -fmad=false), so `score < bestScore` / `score == bestScore` decide identically.
 // Output: a float64 ACTION ROW per env, [lx, ly, 0, lx+x, ly+y, 0, 0, 0, 1], which LeafNode2Action (C:bin3D.py:151-167)
@@ -12,7 +12,7 @@
 // raises, so the row is [W+1, 0, 0, W+1, 0, 0, 0, 0, 1] — Space.drop_box rejects it on its bounds test (C:space.py:336)
 // and pct_step ends the episode with the same counter / ratio.
 //
-// Included at the end of pct_continuous.cu (same translation unit: it reuses GeomC / rest_height_c / CEnv).
+// Included at the end of pct_continuous.cu (same translation unit: it reuses GeomC / CEnv).
 #pragma once
 
 namespace pct {
@@ -31,28 +31,6 @@ __device__ __forceinline__ void heur_rot_c(const double nb[3], int rot, double &
 
 struct HCandC { double sx, sy, sz, lx, ly, ex, ey, ez; bool valid; };
 
-// Space.drop_box_virtual(dims, (lx, ly), False, density, setting, returnH=True) + check_box (C:space.py:380-439) of ONE placement:
-// for the batched queries (pctc_query_kernel).  It is the PCT_H_QUERY_ branch below, expression for expression; that branch keeps
-// its own inline copy because routing it through this function changes the register allocation of pctc_heuristic_kernel, and
-// tests/test_gpu_queries.py pins the two paths to each other.  mh is interSect2D's max_h (C:space.py:391), reported whatever the
-// verdict.  Raised capacity flags go to `fl` (the callers do not OR them into the env).
-template <bool STAB>
-__device__ __forceinline__ int query_placement_c(const CParams &p, const double (*box)[6], int n_box, const GeomC &g, EdgePool &pool, BigScratch *big,
-                                                 int *lock, double sx, double sy, double sz, double lx, double ly, double den, double &mh, int &fl) {
-    bool chk = !(lx + sx - 1e-6 > p.W || ly + sy - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
-    mh = rest_height_c(box, 0, n_box, 1, lx, ly, lx + sx, ly + sy);
-    if (mh < 0) mh = 0.0;
-    if (mh + sz - 1e-6 > p.H) chk = false;
-    int feas;
-    if (!chk) feas = 0;
-    else if (!STAB || fabs(mh) < 1e-6) feas = 1;
-    else {
-        NodeC root{lx, ly, mh, sx, sy, sz, sx * sy * sz * den};
-        feas = stability_check<false, GeomC>(g, root, pool, big, lock, 0, fl) != 0;
-    }
-    return feas;
-}
-
 // enumeration index -> placement: EMS (list order; OnlineBPH: deep-bottom-left order) x orientation, at the EMS origin
 __device__ __forceinline__ HCandC heur_decode_c(int code, int c, const double (*ems)[6], const uint16_t *ord, const double nb[3], int R) {
     HCandC k;
@@ -65,20 +43,22 @@ __device__ __forceinline__ HCandC heur_decode_c(int code, int c, const double (*
     return k;
 }
 
+// 8 / 12 blocks per SM: 128 / 80 registers.  Without the bound the instantiation without a stability test takes 86 registers (11 blocks
+// per SM) and its selection is about 10 % slower on the H100 (scratch/heur_bench_cont.py, setting 2: LSAH 0.127 -> 0.140 ms at 4096 envs)
 template <bool STAB>
-__global__ void __launch_bounds__(64) pctc_heuristic_kernel(const CParams p, const HParamsC hp) {
+__global__ void __launch_bounds__(64, STAB ? 8 : 12) pctc_heuristic_kernel(const CParams p, const HParamsC hp) {
     __shared__ uint16_t ord[CE_MAX];
     __shared__ int c_feas[64];
     __shared__ double c_score[64];
     __shared__ int lock, stop;
     const int tid = threadIdx.x, lane = tid & 31, code = hp.code;
-    const int e = code == PCT_H_QUERY_ ? hp.q_env : blockIdx.x;
+    const int e = blockIdx.x;
     CEnv *ev = p.env + e;
     const CHdr &h = ev->h;
     if (tid == 0) { lock = 0; stop = 0; }
     const double nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
     const int n_ems = h.n_ems, n_box = h.n_box, R = p.setting == 2 ? 6 : 2;
-    const double den = code == PCT_H_QUERY_ ? hp.q_den : h.next_den;
+    const double den = h.next_den;
     if (code == PCT_H_ONLINEBPH) {  // sorted(EMS, key=(z, y, x)) — stable (heuristic.py:383-384); all-zero rows are skipped (:395-396)
         for (int i = tid; i < n_ems; i += 64) {
             const double *a = ev->ems[i];
@@ -96,25 +76,6 @@ __global__ void __launch_bounds__(64) pctc_heuristic_kernel(const CParams p, con
     EdgePool pool{ev->e_lower, ev->e_next, ev->e_off, ev->first_in, ev->last_in, ev->e_st, ev->e_st, h.n_edge,
                   ev->poly_off, &ev->poly[0][0], &ev->poly[0][0], h.n_poly};
     int fl = 0;
-    if (code == PCT_H_QUERY_) {  // one Space.drop_box_virtual(..., returnH=True) call (C:space.py:380-425) for the single-env facade
-        if (tid == 0) {
-            const double sx = hp.q[0], sy = hp.q[1], sz = hp.q[2], lx = hp.q[3], ly = hp.q[4];
-            bool chk = !(lx + sx - 1e-6 > p.W || ly + sy - 1e-6 > p.L) && !(lx + 1e-6 < 0 || ly + 1e-6 < 0);
-            double mh = rest_height_c(ev->box, 0, n_box, 1, lx, ly, lx + sx, ly + sy);
-            if (mh < 0) mh = 0.0;
-            if (mh + sz - 1e-6 > p.H) chk = false;
-            int feas;
-            if (!chk) feas = 0;
-            else if (!STAB || fabs(mh) < 1e-6) feas = 1;
-            else {
-                NodeC root{lx, ly, mh, sx, sy, sz, sx * sy * sz * den};
-                feas = stability_check<false, GeomC>(g, root, pool, &ev->big, &lock, 0, fl) != 0;
-            }
-            hp.q_out[0] = (double)feas;
-            hp.q_out[1] = mh;
-        }
-        return;
-    }
     const int n_c = n_ems * R;
     // LSAH footprint state (heuristic.py:146-147, 217-220); a fresh episode (no box placed yet) starts from the empty footprint
     double maxX = 0, maxY = 0, minX = p.W, minY = p.L;
@@ -133,19 +94,7 @@ __global__ void __launch_bounds__(64) pctc_heuristic_kernel(const CParams p, con
         double mh = 0, score = 0;
         if (c < n_c) {
             const HCandC k = heur_decode_c(code, c, ev->ems, ord, nb, R);
-            if (k.valid) {
-                // Space.drop_box_virtual + check_box (C:space.py:380-439), as in pctc_feas_emit_kernel
-                bool chk = !(k.lx + k.sx - 1e-6 > p.W || k.ly + k.sy - 1e-6 > p.L) && !(k.lx + 1e-6 < 0 || k.ly + 1e-6 < 0);
-                mh = rest_height_c(ev->box, 0, n_box, 1, k.lx, k.ly, k.lx + k.sx, k.ly + k.sy);
-                if (mh < 0) mh = 0.0;
-                if (mh + k.sz - 1e-6 > p.H) chk = false;
-                if (!chk) feas = 0;
-                else if (!STAB || fabs(mh) < 1e-6) feas = 1;
-                else {
-                    NodeC root{k.lx, k.ly, mh, k.sx, k.sy, k.sz, k.sx * k.sy * k.sz * den};
-                    feas = stability_check<false, GeomC>(g, root, pool, &ev->big, &lock, 0, fl) != 0;
-                }
-            }
+            if (k.valid) feas = place_virtual_c<STAB>(p, g, pool, &ev->big, &lock, k.sx, k.sy, k.sz, k.lx, k.ly, den, mh, fl);
             if (feas) {
                 if (code == PCT_H_LSAH) {  // heuristic.py:196-200
                     const double ex = fmax(k.lx + k.sx, maxX) - fmin(k.lx, minX), ey = fmax(k.ly + k.sy, maxY) - fmin(k.ly, minY);
@@ -206,9 +155,9 @@ __global__ void __launch_bounds__(64) pctc_heuristic_kernel(const CParams p, con
 }
 
 // Batched placement queries (pct_query_placements_f64): a block of 64 threads owns one row (k placements of one env, read in
-// place like pctc_heuristic_kernel does), one thread per placement of the current 64-chunk, answered by query_placement_c.  Nothing
-// is written back to the env.  Envs within one launch are distinct (caller's contract): stability_check uses the env's `big`
-// scratch under the block's lock.
+// place like pctc_heuristic_kernel does), one thread per placement of the current 64-chunk, answered by place_virtual_c
+// (pct_block.cuh); pct_query_placement_f64 asks one row of one placement here.  Nothing is written back to the env.  Envs
+// within one launch are distinct (caller's contract): stability_check uses the env's `big` scratch under the block's lock.
 template <bool STAB>
 __global__ void __launch_bounds__(64) pctc_query_kernel(const CParams p, const QParams q) {
     __shared__ int lock;
@@ -240,17 +189,15 @@ __global__ void __launch_bounds__(64) pctc_query_kernel(const CParams p, const Q
         const double *x = qv + (row + j) * 5;
         const double den = q.density ? q.density[row + j] : h.next_den;
         double mh;
-        const int feas = query_placement_c<STAB>(p, ev->box, n_box, g, pool, &ev->big, &lock, x[0], x[1], x[2], x[3], x[4], den, mh, fl);
+        const int feas = place_virtual_c<STAB>(p, g, pool, &ev->big, &lock, x[0], x[1], x[2], x[3], x[4], den, mh, fl);
         if (q.feasible) q.feasible[row + j] = (uint8_t)feas;
         if (rest) rest[row + j] = mh;
     }
 }
 
-// the baselines over the batch, or (hp.code == PCT_H_QUERY_) the single placement query of env hp.q_env
 cudaError_t launch_heuristic_continuous(const CParams &p, const HParamsC &hp, cudaStream_t st) {
-    const int blocks = hp.code == PCT_H_QUERY_ ? 1 : p.n_envs;
-    if (p.setting == 2) pctc_heuristic_kernel<false><<<blocks, 64, 0, st>>>(p, hp);
-    else pctc_heuristic_kernel<true><<<blocks, 64, 0, st>>>(p, hp);
+    if (p.setting == 2) pctc_heuristic_kernel<false><<<p.n_envs, 64, 0, st>>>(p, hp);
+    else pctc_heuristic_kernel<true><<<p.n_envs, 64, 0, st>>>(p, hp);
     return cudaGetLastError();
 }
 

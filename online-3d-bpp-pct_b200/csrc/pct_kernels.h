@@ -243,26 +243,19 @@ constexpr int PCT_OPT_DELTA = 1, PCT_OPT_ALIAS = 2, PCT_OPT_K3_BLOCK = 4, PCT_OP
 
 // heuristic baselines (pct_heuristics.cuh)
 struct HParams {
-    int code;                // enum pct_heuristic; PCT_H_QUERY_ = single placement query
+    int code;                // enum pct_heuristic
     float *rows;             // (n_envs, 9) action rows
     int32_t *hstate;         // (n_envs, 4) LSAH footprint of the packed items: maxX, maxY, minX, minY (heuristic.py:146-147)
     uint64_t seed;           // RANDOM
     int64_t t;
-    int q_env, q[5];         // query: handle-local env, oriented dims, lx, ly
-    double q_den;
-    int32_t *q_out;          // [feasible, rest height, W*L height map after the placement]
 };
 // continuous domain (pct_heuristics_continuous.cuh): LSAH / OnlineBPH / BR, float64 rows and footprint state
 struct HParamsC {
     int code;
     double *rows;            // (n_envs, 9) float64 action rows
     double *hstate;          // (n_envs, 4) LSAH footprint: maxX, maxY, minX, minY
-    int q_env;               // PCT_H_QUERY_: handle-local env, oriented sizes + position, density, result [feasible, rest height]
-    double q[5], q_den;
-    double *q_out;
 };
-constexpr int PCT_H_QUERY_ = 7;
-constexpr int HEUR_SIDE_MAX = 32;  // static height map of the heuristic kernel (single discrete query: W, L <= 32; HM / MACS / RANDOM above it: BIG instantiation)
+constexpr int HEUR_SIDE_MAX = 32;  // static height map of the heuristic kernel (HM / MACS / RANDOM above it: BIG instantiation); the single discrete query's limit
 cudaError_t launch_heuristic_discrete(const DParams &p, const HParams &hp, cudaStream_t st);
 cudaError_t prepare_heuristic_big();  // pct_create of a discrete handle with W or L > HEUR_SIDE_MAX
 

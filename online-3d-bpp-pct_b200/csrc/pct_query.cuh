@@ -1,16 +1,15 @@
 // Batched placement queries and height maps of the discrete env (pct_query_placements / pct_height_maps, include/pct_b200.h).
 //
-// Queries: a block of FEAS_THREADS owns one row (n_rows x k placements of one env).  It stages the env exactly like
-// pct_heuristic_kernel (TMA bulk copy of DEnvHot, then the first load edges and polygon vertices when the setting has a
-// stability test) and gives each placement of the current FEAS_THREADS-chunk its own thread, which answers it with
-// query_placement_d — the code of the single query, so every answer is that of pct_query_placement.  Nothing is written
-// back to the env: capacity flags raised by stability_check stay in the thread, as in the single query.  Envs within one
-// launch are distinct (caller's contract), because stability_check uses the env's `big` scratch under the block's lock.
+// Queries: a block of FEAS_THREADS owns one row (n_rows x k placements of one env).  It stages the env (stage_env_d,
+// pct_block.cuh) and gives each placement of the current FEAS_THREADS-chunk its own thread, which answers it with the
+// placement test of every discrete kernel, place_virtual_d.  pct_query_placement asks one row of one placement here.  Nothing
+// is written back to the env: capacity flags raised by stability_check stay in the thread.  Envs within one launch are
+// distinct (caller's contract), because stability_check uses the env's `big` scratch under the block's lock.
 //
 // Height maps: a block per env stages the placed boxes and gives each cell its own thread, with the Space.plain expression
 // of pct_heuristic_kernel; the map goes straight to global memory, so the container has no side limit here.
 //
-// Included at the end of pct_discrete.cu (same translation unit: it reuses GeomD / rest_height / the staging layout).
+// Included at the end of pct_discrete.cu (same translation unit: it reuses FEAS_THREADS and rest_height).
 #pragma once
 
 namespace pct {
@@ -19,7 +18,7 @@ constexpr int HMAP_THREADS = 128;
 
 template <bool STAB>
 __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_query_kernel(const DParams p, const QParams q) {
-    __shared__ __align__(16) unsigned char sm[K3_SMEM];
+    __shared__ __align__(16) StageD sm;
     const int tid = threadIdx.x, r = blockIdx.x, K = q.k;
     const int e = q.env ? q.env[r] : r;
     const size_t row = (size_t)r * K;
@@ -31,40 +30,8 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_query_kernel(const DParam
         }
         return;
     }
-    DEnvHot *hot = (DEnvHot *)sm;
-    uint64_t *mbar = (uint64_t *)(sm + sizeof(DEnvHot) + NL_MAX * 12);
-    int *lock = (int *)(mbar + 1);
-    Stack4 *st_sm = (Stack4 *)(sm + sizeof(DEnvHot) + NL_MAX * 12 + 64);
-    double *poly_sm = (double *)(st_sm + EDGE_STAGE);
-    DEnvHot *ghot = p.hot + e;
-    DEnvCold *cold = p.cold + e;
-    if (tid == 0) {
-        *lock = 0;
-        mbar_init(mbar, 1);
-        fence_proxy_async();
-    }
-    __syncthreads();
-    if (tid == 0) {
-        mbar_expect_tx(mbar, (uint32_t)sizeof(DEnvHot));
-        tma_load_1d(hot, ghot, (uint32_t)sizeof(DEnvHot), mbar);
-    }
-    mbar_wait(mbar, 0);
-    __syncthreads();
-    const DHdr &h = hot->h;
-    if (STAB && h.n_edge > 0) {
-        const uint32_t bytes = (uint32_t)min(h.n_edge, EDGE_STAGE) * (uint32_t)sizeof(Stack4);
-        const uint32_t pbytes = (uint32_t)min(h.n_poly, POLY_STAGE) * 16u;
-        if (tid == 0) {
-            mbar_expect_tx(mbar, bytes + pbytes);
-            tma_load_1d(st_sm, cold->e_st, bytes, mbar);
-            if (pbytes) tma_load_1d(poly_sm, cold->poly, pbytes, mbar);
-        }
-        mbar_wait(mbar, 1);
-    }
-    const int n_box = h.n_box;
-    GeomD g{hot->box, n_box, p.setting == 3 ? cold->density : nullptr};
-    EdgePool pool{hot->e_lower, hot->e_next, hot->e_off, hot->first_in, hot->last_in, cold->e_st, st_sm, h.n_edge,
-                  hot->poly_off, &cold->poly[0][0], poly_sm, h.n_poly};
+    StagedD sd = stage_env_d<STAB>(sm, p, e, false);
+    const double next_den = sm.hot.h.next_den;
     int fl = 0;  // not ORed into the env: a query leaves the env as it was
     const int32_t *qv = (const int32_t *)q.q;
 #pragma unroll 1
@@ -72,9 +39,11 @@ __global__ void __launch_bounds__(FEAS_THREADS, 4) pct_query_kernel(const DParam
         const int j = base + tid;
         if (j >= K) break;
         const int32_t *x = qv + (row + j) * 5;
-        const double den = q.density ? q.density[row + j] : h.next_den;
-        int mh;
-        const int feas = query_placement_d<STAB>(hot, n_box, g, pool, &cold->big, lock, p.W, p.L, p.H, x[0], x[1], x[2], x[3], x[4], den, mh, fl);
+        const int sx = x[0], sy = x[1], sz = x[2], lx = x[3], ly = x[4];
+        const double den = q.density ? q.density[row + j] : next_den;
+        int feas = 0, mh = 0;  // a position outside [0, W) x [0, L) or a zero footprint: infeasible, rest height 0
+        if (lx >= 0 && ly >= 0 && lx < p.W && ly < p.L && sx > 0 && sy > 0)
+            feas = place_virtual_d<STAB>(p, sd.g, sd.pool, &p.cold[e].big, &sm.lock, sx, sy, sz, lx, ly, den, mh, fl);
         if (q.feasible) q.feasible[row + j] = (uint8_t)feas;
         if (rest) rest[row + j] = mh;
     }
