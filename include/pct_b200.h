@@ -326,6 +326,36 @@ int pct_expand_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, c
  * than the step's forces full row writes. */
 int pct_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream);
 
+/* pct_step for chosen envs of the batch, at a cost that scales with their number: a search that expands one node per tree, actors whose
+ * policies answer at different times (EnvPool's send(action, env_id) / recv), an evaluation that stops stepping envs whose episode quota
+ * is used up.  Exactly one of d_env / d_mask is non-NULL, as for pct_reset_envs:
+ *   d_env : n distinct env indices (caller's contract); an index outside [0, n_envs) is skipped.
+ *   d_mask: n_envs bytes, n == n_envs; env e steps iff d_mask[e] != 0.  For graph capture, where the host does not know how many envs
+ *           step.  The call copies the mask into the handle before its first kernel, so the selection is the mask as it stood when the
+ *           call's work began: it may be one of the call's own outputs, e.g. the d_done of the previous step passed as is.
+ * The other arguments are pct_step's, with its full per-env buffers: a selected env e reads action row e / d_leaf_idx[e] and writes
+ * observation row e, d_reward[e], d_done[e] and d_info[e].  Entries of envs not selected are neither read nor written, and their
+ * records are not touched.  A selected env's step is exactly pct_step's for that env (auto-reset of a finished env included, unless
+ * no_auto_reset), so its trajectory does not depend on which envs step with it (until it raises PCT_FLAG_CAND_OVERFLOW: the stability
+ * walks of one call share a pool sized by n_envs, and past an overflow a step depends on what else ran, as in pct_step); the delta-row
+ * contract of pct_step holds per env.
+ * A selected step runs in env order without programmatic overlap, on the caller's stream whatever PCT_B200_GROUPS says.
+ * Enqueue only: no host synchronisation, no allocation (CUDA-graph capturable).  n == 0 (d_env): no-op.  Errors: PCT_ERR_STATE before
+ * pct_reset or without an item source; PCT_ERR_INVALID when both or neither of d_env / d_mask are given, for n < 0, for a mask with
+ * n != n_envs, without d_obs / d_reward / d_done, and unless exactly one of d_actions / d_leaf_idx is given. */
+int pct_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, const void *d_actions, int32_t action_f64,
+                  const int32_t *d_leaf_idx, void *d_obs, float *d_reward, uint8_t *d_done, pct_step_info *d_info, void *stream);
+
+/* pct_reset_envs re-expanding only the selected envs: the same arguments, errors and result for a selected env (its rows of d_obs, its
+ * d_info record, its env record), but envs not selected are not re-expanded and their rows and records are not written.  The cost scales
+ * with the selection; the gym loop becomes pct_step -> pct_reset_envs_only(d_mask = d_done). */
+int pct_reset_envs_only(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream);
+
+/* pct_set_items re-expanding only the listed envs: the same arguments, errors and result for a listed env (d_env NULL: envs 0 .. n-1),
+ * but envs not listed are not re-expanded and their rows and records are not written.  The envs of one call must be distinct. */
+int pct_set_items_only(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
+                       pct_step_info *d_info, void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

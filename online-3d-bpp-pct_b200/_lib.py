@@ -66,7 +66,8 @@ EXPORTS = ["pct_create", "pct_destroy", "pct_last_error", "pct_set_item_set", "p
            "pct_state_bytes_per_env", "pct_kernel_launches", "pct_version", "pct_profile_enable", "pct_profile_read", "pct_heuristic_actions",
            "pct_heuristic_actions_f64", "pct_query_placement", "pct_query_placement_f64",
            "pct_snapshot_bytes", "pct_snapshot", "pct_restore", "pct_query_placements", "pct_query_placements_f64", "pct_height_maps",
-           "pct_preview_items", "pct_set_items", "pct_expand_items", "pct_reset_envs", "pct_get_support_graph"]
+           "pct_preview_items", "pct_set_items", "pct_expand_items", "pct_reset_envs", "pct_get_support_graph",
+           "pct_step_envs", "pct_reset_envs_only", "pct_set_items_only"]
 
 
 def build(verbose=False):
@@ -128,5 +129,8 @@ def lib():
     L.pct_set_items.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     L.pct_expand_items.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp]
     L.pct_reset_envs.argtypes = [vp, vp, i32, vp, vp, vp, vp]
+    L.pct_step_envs.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp]
+    L.pct_reset_envs_only.argtypes = [vp, vp, i32, vp, vp, vp, vp]
+    L.pct_set_items_only.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     _lib = L
     return L

@@ -109,14 +109,34 @@ class PctBatch(object):
         self._check(self.L.pct_set_trajectory_length(self.h, int(traj_len)), "pct_set_trajectory_length")
 
     # -- device-resident API -------------------------------------------------------------------------------
-    def reset(self, out=None, env_idx=None, mask=None, info=None):
+    def _selection(self, env_idx, mask, what):
+        """(idx, mask, n) of a selection of envs: exactly one of env_idx (distinct indices) / mask ((n_envs,) bool / uint8 tensor)"""
+        if env_idx is not None and mask is not None:
+            raise PctError("%s: pass env_idx or mask, not both" % what)
+        if not self.did_reset:
+            raise PctError("%s(env_idx / mask) before the first reset() of the batch" % what)
+        if mask is None:
+            idx = self._index(env_idx, "env_idx")
+            return idx, None, int(idx.numel())
+        if not torch.is_tensor(mask):
+            mask = torch.as_tensor(np.asarray(mask))
+        if mask.dtype not in (torch.bool, torch.uint8) or tuple(mask.shape) != (self.n_envs,):
+            raise PctError("%s mask must be an (n_envs,) = (%d,) bool or uint8 tensor" % (what, self.n_envs))
+        m = mask.to(self.device).contiguous()
+        if m.dtype == torch.bool:
+            m = m.view(torch.uint8)  # same bytes (0 / 1): no copy, so a captured graph reads the caller's tensor
+        return None, m, self.n_envs
+
+    def reset(self, out=None, env_idx=None, mask=None, info=None, whole_batch=True):
         """Without env_idx / mask: reset every env (VecEnv.reset()).  With one of them: env.reset() for the chosen envs only
         (pct_reset_envs, include/pct_b200.h), enqueued on the current stream (graph-capturable) after a first full reset.  env_idx: distinct
         env indices (indices outside [0, n_envs) are skipped); mask: an (n_envs,) bool / uint8 tensor, e.g. the `done` of the last step,
         so `reset(mask=done)` gives gym semantics to a batch built with auto_reset=False.  Every env of the batch is re-expanded (envs not
         chosen come out unchanged) and the complete observation goes to `out` (default: the batch's own observation buffer, under the
         delta-row contract of step), which is returned: clone() a terminal observation before resetting over it.  info: optional
-        (n_envs, 8) int32 tensor for the pct_step_info records of the new expansions.  An empty env_idx enqueues nothing."""
+        (n_envs, 8) int32 tensor for the pct_step_info records of the new expansions.  An empty env_idx enqueues nothing.
+        whole_batch=False (pct_reset_envs_only): only the chosen envs are re-expanded, and only their rows of `out` and of `info` are
+        written, at a cost in proportion to the chosen envs."""
         if env_idx is None and mask is None:
             if info is not None:
                 raise PctError("reset: info is written by a reset of chosen envs (env_idx or mask) only")
@@ -124,39 +144,29 @@ class PctBatch(object):
             self._check(self.L.pct_reset(self.h, C.c_void_p(obs.data_ptr()), self._stream()), "pct_reset")
             self.did_reset = True
             return obs
-        if env_idx is not None and mask is not None:
-            raise PctError("reset: pass env_idx or mask, not both")
-        if not self.did_reset:
-            raise PctError("reset(env_idx / mask) before the first reset() of the batch")
+        idx, m, n = self._selection(env_idx, mask, "reset")
         obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "reset out")
         if info is not None:
             info = self._out(info, (self.n_envs, 8), torch.int32, "reset info")
-        idx = m = None
-        if mask is not None:
-            if not torch.is_tensor(mask):
-                mask = torch.as_tensor(np.asarray(mask))
-            if mask.dtype not in (torch.bool, torch.uint8) or tuple(mask.shape) != (self.n_envs,):
-                raise PctError("reset mask must be an (n_envs,) = (%d,) bool or uint8 tensor" % self.n_envs)
-            m = mask.to(self.device).contiguous()
-            if m.dtype == torch.bool:
-                m = m.view(torch.uint8)  # same bytes (0 / 1): no copy, so a captured graph reads the caller's tensor
-            n = self.n_envs
-        else:
-            idx = self._index(env_idx, "env_idx")
-            n = int(idx.numel())
-            if n == 0:
-                return obs
+        if n == 0:
+            return obs
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-        self._check(self.L.pct_reset_envs(self.h, ptr(idx), n, ptr(m), C.c_void_p(obs.data_ptr()), ptr(info), self._stream()),
-                    "pct_reset_envs")
+        fn, what = (self.L.pct_reset_envs, "pct_reset_envs") if whole_batch else (self.L.pct_reset_envs_only, "pct_reset_envs_only")
+        self._check(fn(self.h, ptr(idx), n, ptr(m), C.c_void_p(obs.data_ptr()), ptr(info), self._stream()), what)
         return obs
 
-    def step(self, actions=None, leaf_idx=None, out=None):
+    def step(self, actions=None, leaf_idx=None, out=None, env_idx=None, mask=None):
         """actions: (N,9) float32/float64 CUDA tensor of leaf rows, or leaf_idx: (N,) int32 CUDA tensor.
         Returns (obs, reward(N,), done(N,) uint8, info(N,8) int32 raw pct_step_info records) — all on the GPU.
         NOTE: without `out`, the four tensors are the library-owned buffers, rewritten IN PLACE by the next reset / step (zero-copy; and with the
         delta observation rows, include/pct_b200.h, the observation buffer must not be modified by the caller).  Keep a result across steps with
-        .clone(), or pass your own `out` buffers (e.g. a rollout storage, GraphedRollout); PctVecEnv hands out fresh observation tensors."""
+        .clone(), or pass your own `out` buffers (e.g. a rollout storage, GraphedRollout); PctVecEnv hands out fresh observation tensors.
+        env_idx (distinct env indices; indices outside [0, n_envs) are skipped) or mask ((n_envs,) bool / uint8 tensor): step only those envs
+        (pct_step_envs), at a cost in proportion to them.  actions / leaf_idx keep their full size and only the chosen envs' rows are read;
+        only the chosen envs' rows of the four returned buffers are written.  An empty env_idx enqueues nothing."""
+        sel = env_idx is not None or mask is not None
+        if sel:
+            idx, m, n = self._selection(env_idx, mask, "step")
         obs = self._obs if out is None else out
         a_ptr, i_ptr, f64 = None, None, 0
         if actions is not None:
@@ -168,7 +178,16 @@ class PctBatch(object):
             a_ptr, f64 = C.c_void_p(actions.data_ptr()), int(actions.dtype == torch.float64)
         else:
             leaf_idx = leaf_idx.to(torch.int32).contiguous()
+            if sel and tuple(leaf_idx.shape) != (self.n_envs,):
+                raise PctError("leaf_idx must have shape (n_envs,)")
             i_ptr = C.c_void_p(leaf_idx.data_ptr())
+        if sel:
+            if n:
+                ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+                self._check(self.L.pct_step_envs(self.h, ptr(idx), n, ptr(m), a_ptr, f64, i_ptr, C.c_void_p(obs.data_ptr()),
+                                                 C.c_void_p(self._rew.data_ptr()), C.c_void_p(self._done.data_ptr()),
+                                                 C.c_void_p(self._info.data_ptr()), self._stream()), "pct_step_envs")
+            return obs, self._rew, self._done, self._info
         self._check(self.L.pct_step(self.h, a_ptr, f64, i_ptr, C.c_void_p(obs.data_ptr()), C.c_void_p(self._rew.data_ptr()),
                                     C.c_void_p(self._done.data_ptr()), C.c_void_p(self._info.data_ptr()), self._stream()), "pct_step")
         return obs, self._rew, self._done, self._info
@@ -359,14 +378,15 @@ class PctBatch(object):
                                              C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_preview_items")
         return out
 
-    def set_items(self, items, env_idx=None, density=None, out=None, info=None):
+    def set_items(self, items, env_idx=None, density=None, out=None, info=None, whole_batch=True):
         """Env env_idx[i] (default: env i) <- items[i] as its current item, without consuming a draw, then the leaf expansion of
         cur_observation for it (the reference's `env.next_box = item` + get_possible_position()).  items: (n, 3) sizes, converted to int32
         (discrete) / float64 (continuous); density: (n,) densities (default: keep each env's current density).  EVERY env of the batch is
         re-expanded (envs not listed come out unchanged), and the complete observation goes to `out` (default: the batch's own observation
         buffer, under the delta-row contract of step), which is returned.  info: optional (n_envs, 8) int32 tensor for the pct_step_info
         records (capacity flags of the new expansions, n_leaf, ...).  The envs of one call must be distinct.  No items (n == 0): nothing is
-        enqueued and nothing is written."""
+        enqueued and nothing is written.  whole_batch=False (pct_set_items_only): only the listed envs are re-expanded, and only their
+        rows of `out` and of `info` are written."""
         qd = torch.float64 if self.continuous else torch.int32
         if not torch.is_tensor(items):
             items = torch.as_tensor(np.asarray(items))
@@ -390,8 +410,8 @@ class PctBatch(object):
         if info is not None:
             info = self._out(info, (self.n_envs, 8), torch.int32, "set_items info")
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
-        self._check(self.L.pct_set_items(self.h, ptr(idx), n, ptr(it), ptr(den), C.c_void_p(obs.data_ptr()), ptr(info), self._stream()),
-                    "pct_set_items")
+        fn, what = (self.L.pct_set_items, "pct_set_items") if whole_batch else (self.L.pct_set_items_only, "pct_set_items_only")
+        self._check(fn(self.h, ptr(idx), n, ptr(it), ptr(den), C.c_void_p(obs.data_ptr()), ptr(info), self._stream()), what)
         return obs
 
     def expand_items(self, items, env_idx=None, density=None, out=None):

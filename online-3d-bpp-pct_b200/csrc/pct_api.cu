@@ -192,6 +192,7 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
     const bool disc = cfg->domain == PCT_DISCRETE;
     if (e == cudaSuccess) e = cudaMalloc(&h->d_ready, sizeof(int32_t) * 2 * (size_t)n_envs);
     if (e == cudaSuccess) e = cudaMemset(h->d_ready, 0, sizeof(int32_t) * 2 * (size_t)n_envs);
+    if (e == cudaSuccess) e = cudaMalloc(&h->d_sel_mask, (size_t)n_envs);
     if (disc) {
         if (e == cudaSuccess) e = cudaMalloc(&h->d_hot, sizeof(DEnvHot) * (size_t)n_envs);
         if (e == cudaSuccess) e = cudaMalloc(&h->d_cold, sizeof(DEnvCold) * (size_t)n_envs);
@@ -236,7 +237,7 @@ void pct_destroy(pct_handle h) {
     cudaFree(h->d_order);
     cudaFree(h->d_walkq); cudaFree(h->d_walk_ctr); cudaFree(h->d_contq); cudaFree(h->d_cont_ctr); cudaFree(h->d_piece_ready); cudaFree(h->d_walk_pend);
     cudaFree(h->d_hstate); cudaFree(h->d_hstate_c); cudaFree(h->d_query_c); cudaFree(h->d_query); cudaFree(h->d_aux);
-    cudaFree(h->d_ready);
+    cudaFree(h->d_ready); cudaFree(h->d_sel_mask);
     cudaFree(h->d_hot); cudaFree(h->d_cold); cudaFree(h->d_item_set); cudaFree(h->d_stream);
     cudaFree(h->d_obs); cudaFree(h->d_act); cudaFree(h->d_idx); cudaFree(h->d_rew); cudaFree(h->d_done); cudaFree(h->d_info);
     for (cudaEvent_t ev : h->prof_ev) if (ev) cudaEventDestroy(ev);
@@ -291,9 +292,11 @@ static void begin_obs(pct_handle h, const void *obs) {
     h->tracked_obs = obs;
 }
 
-// pre non-null (pct_set_items / pct_reset_envs): its kernel replaces the apply kernel; whole batch, non-overlapped order, env order (no LPT parity flip)
+// pre non-null (pct_set_items / pct_reset_envs): its kernel replaces the apply kernel; whole batch, non-overlapped order, env order (no LPT parity flip).
+// sel non-null (pct_step_envs and the _only calls): the selected envs of the whole batch (off = 0, cnt = n_envs), in the same launch order as pre
 static int launch_range(pct_handle h, int mode, int off, int cnt, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs,
-                        float *rew, uint8_t *done, pct_step_info *info, cudaStream_t gs, bool whole_batch, const PreKernel *pre = nullptr) {
+                        float *rew, uint8_t *done, pct_step_info *info, cudaStream_t gs, bool whole_batch, const PreKernel *pre = nullptr,
+                        const EnvSel *sel = nullptr) {
     const size_t osz = h->cfg.obs_dtype == PCT_F64 ? 8 : 4, asz = action_f64 ? 8 : 4;
     DParams p = discrete_params(h, off, cnt);
     p.actions = actions ? (const char *)actions + (size_t)off * 9 * asz : nullptr; p.action_f64 = action_f64;
@@ -301,10 +304,10 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
     p.obs = (char *)obs + (size_t)off * h->obs_len * osz;
     p.reward = rew ? rew + off : nullptr; p.done = done ? done + off : nullptr; p.info = info ? info + off : nullptr; p.mode = mode;
     p.dbg = (long long *)h->dbg;
-    p.order = (h->lpt && whole_batch && !pre) ? h->d_order : nullptr;
+    p.order = (h->lpt && whole_batch && !pre && !sel) ? h->d_order : nullptr;
     // overlapped launch mode: not while a CUDA graph is being captured (the epoch would be frozen into the graph and a replay
     // would find the flags of the previous replay already set), not under the per-kernel profiler, not with the LPT permutation
-    if (h->overlap && !h->prof_on && !capturing(gs) && !pre) {
+    if (h->overlap && !h->prof_on && !capturing(gs) && !pre && !sel) {
         p.ready = h->d_ready + 2 * (size_t)off;
         p.epoch = ++h->epoch;
     }
@@ -316,7 +319,7 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
     if (h->k3_block) p.opt |= PCT_OPT_K3_BLOCK;
     if (h->no_emit_pdl) p.opt |= PCT_OPT_NO_EMIT_PDL;
     cudaEvent_t *prof = nullptr;
-    if (h->prof_on && mode == 1 && whole_batch && !pre) {
+    if (h->prof_on && mode == 1 && whole_batch && !pre && !sel) {
         if ((size_t)(h->prof_steps + 1) * 4 > h->prof_ev.size()) {
             const size_t old = h->prof_ev.size();
             h->prof_ev.resize(old + 4096, nullptr);
@@ -326,22 +329,22 @@ static int launch_range(pct_handle h, int mode, int off, int cnt, const void *ac
         h->prof_steps++;
     }
     p.walk = walk_pools<WalkItem>(h, off, cnt);
-    if (pre) CK(h, pre->items ? launch_set_items_discrete(p, *pre->items, gs) : launch_reset_envs_discrete(p, *pre->reset, gs));
-    else CK(h, launch_discrete(p, gs, prof));
+    if (pre) CK(h, pre->items ? launch_set_items_discrete(p, *pre->items, gs, sel) : launch_reset_envs_discrete(p, *pre->reset, gs, sel));
+    else CK(h, launch_discrete(p, gs, prof, true, sel));
     h->launches += discrete_kernels_per_step(p);
     return PCT_OK;
 }
 
 // the continuous step over the whole batch on stream st; pre as in launch_range
 static int launch_continuous_step(pct_handle h, int mode, const void *actions, int action_f64, const int32_t *leaf_idx, void *obs, float *rew,
-                                  uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre = nullptr) {
+                                  uint8_t *done, pct_step_info *info, cudaStream_t st, const PreKernel *pre = nullptr, const EnvSel *sel = nullptr) {
     CParams p = continuous_params(h);
     p.actions = actions; p.action_f64 = action_f64; p.leaf_idx = leaf_idx;
     p.obs = obs; p.reward = rew; p.done = done; p.info = info; p.mode = mode;
     // overlapped launch mode (off by default: measured slower in this domain): not while a CUDA graph is being captured (see launch_range);
     // the emit kernel's programmatic launch neither
     const bool cap = capturing(st);
-    if (h->overlap_cont && !cap && !pre) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
+    if (h->overlap_cont && !cap && !pre && !sel) { p.ready = h->d_ready; p.epoch = ++h->epoch; }
     p.aux = h->d_aux;
     int opt = (h->alias_mode ? PCT_OPT_ALIAS : 0) | (cap ? PCT_OPT_NO_EMIT_PDL : 0) | (h->cont_pre ? PCT_OPT_CONT_PRE : 0);
     if (h->d_walkq) {
@@ -350,8 +353,8 @@ static int launch_continuous_step(pct_handle h, int mode, const void *actions, i
         if (h->obs_delta && h->fill_pending) opt |= PCT_OPT_FILL_PREV;
     }
     h->fill_pending = false;
-    if (pre) CK(h, pre->items ? launch_set_items_continuous(p, opt, *pre->items, st) : launch_reset_envs_continuous(p, opt, *pre->reset, st));
-    else CK(h, launch_continuous(p, opt, st));
+    if (pre) CK(h, pre->items ? launch_set_items_continuous(p, opt, *pre->items, st, sel) : launch_reset_envs_continuous(p, opt, *pre->reset, st, sel));
+    else CK(h, launch_continuous(p, opt, st, true, sel));
     h->launches += continuous_kernels_per_step(p);
     return PCT_OK;
 }
@@ -702,14 +705,81 @@ int pct_expand_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, c
 }
 
 // pct_set_items / pct_reset_envs: the pre-kernel in place of the apply kernel, then the rest of the step's pipeline over the whole batch,
-// on the caller's stream whatever PCT_B200_GROUPS says
-static int launch_pre(pct_handle h, const PreKernel &pre, void *d_obs, pct_step_info *d_info, cudaStream_t st) {
+// on the caller's stream whatever PCT_B200_GROUPS says.  sel non-null (the _only calls): over the selected envs alone
+static int launch_pre(pct_handle h, const PreKernel &pre, void *d_obs, pct_step_info *d_info, cudaStream_t st, const EnvSel *sel = nullptr) {
     CK(h, cudaSetDevice(h->device));
     begin_obs(h, d_obs);
-    if (h->cfg.domain == PCT_CONTINUOUS) return launch_continuous_step(h, 1, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, &pre);
-    const int rc = launch_range(h, 1, 0, h->n_envs, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, true, &pre);
+    if (h->cfg.domain == PCT_CONTINUOUS) return launch_continuous_step(h, 1, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, &pre, sel);
+    const int rc = launch_range(h, 1, 0, h->n_envs, nullptr, 0, nullptr, d_obs, nullptr, nullptr, d_info, st, true, &pre, sel);
     h->fill_pending = false;
     return rc;
+}
+
+// argument checks of a selection (pct_reset_envs, pct_step_envs, pct_reset_envs_only): exactly one of list / mask, n >= 0, a mask of n_envs entries
+static int check_selection(pct_handle h, const char *what, const int32_t *d_env, int32_t n, const uint8_t *d_mask) {
+    if ((d_env == nullptr) == (d_mask == nullptr)) { h->err = std::string(what) + ": pass exactly one of d_env / d_mask"; return PCT_ERR_INVALID; }
+    if (n < 0) { h->err = std::string(what) + ": n must be >= 0"; return PCT_ERR_INVALID; }
+    if (d_mask && n != h->n_envs) { h->err = std::string(what) + ": a mask has n_envs entries (n = " + std::to_string(n) + ")"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = std::string(what) + " before pct_reset"; return PCT_ERR_STATE; }
+    return PCT_OK;
+}
+
+// The selection of a call as its kernels read it.  The mask form is read by every kernel of the pipeline, and the apply kernel writes d_done
+// in between: the mask is copied into the handle's own array first, so that a mask which is one of the call's outputs (the d_done of the
+// previous step, passed as is) selects exactly the envs it named when the call was enqueued.
+static int resolve_selection(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, cudaStream_t st, EnvSel &sel) {
+    sel = EnvSel{d_env, nullptr, n};
+    if (d_mask) {
+        CK(h, cudaMemcpyAsync(h->d_sel_mask, d_mask, (size_t)h->n_envs, cudaMemcpyDeviceToDevice, st));
+        sel.mask = h->d_sel_mask;
+    }
+    return PCT_OK;
+}
+
+int pct_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, const void *d_actions, int32_t action_f64,
+                  const int32_t *d_leaf_idx, void *d_obs, float *d_reward, uint8_t *d_done, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_selection(h, "pct_step_envs", d_env, n, d_mask);
+    if (rc != PCT_OK || n == 0) return rc;
+    if (!d_obs || !d_reward || !d_done) { h->err = "pct_step_envs: d_obs, d_reward and d_done must not be NULL"; return PCT_ERR_INVALID; }
+    if ((d_actions == nullptr) == (d_leaf_idx == nullptr)) { h->err = "pct_step_envs: pass exactly one of d_actions / d_leaf_idx"; return PCT_ERR_INVALID; }
+    rc = check_item_source(h);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    EnvSel sel;
+    rc = resolve_selection(h, d_env, n, d_mask, st, sel);
+    if (rc) return rc;
+    begin_obs(h, d_obs);
+    if (h->cfg.domain == PCT_CONTINUOUS)
+        return launch_continuous_step(h, 1, d_actions, action_f64, d_leaf_idx, d_obs, d_reward, d_done, d_info, st, nullptr, &sel);
+    rc = launch_range(h, 1, 0, h->n_envs, d_actions, action_f64, d_leaf_idx, d_obs, d_reward, d_done, d_info, st, true, nullptr, &sel);
+    h->fill_pending = false;
+    return rc;
+}
+
+int pct_reset_envs_only(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_selection(h, "pct_reset_envs_only", d_env, n, d_mask);
+    if (rc != PCT_OK || n == 0) return rc;
+    if (!d_obs) { h->err = "pct_reset_envs_only: d_obs is NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    EnvSel sel;
+    rc = resolve_selection(h, d_env, n, d_mask, (cudaStream_t)stream, sel);
+    if (rc) return rc;
+    const ResetParams rp{sel.env, n, sel.mask};
+    return launch_pre(h, PreKernel{nullptr, &rp}, d_obs, d_info, (cudaStream_t)stream, &sel);
+}
+
+int pct_set_items_only(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
+                       pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_items(h, "pct_set_items_only", n, 1, d_items, "d_items");
+    if (rc != PCT_OK || n == 0) return rc;
+    if (!d_obs) { h->err = "pct_set_items_only: d_obs is NULL"; return PCT_ERR_INVALID; }
+    const ItemParams ip{d_env, n, 1, d_items, d_density, nullptr};
+    const EnvSel sel{d_env, nullptr, n};
+    return launch_pre(h, PreKernel{&ip, nullptr}, d_obs, d_info, (cudaStream_t)stream, &sel);
 }
 
 int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
@@ -724,11 +794,8 @@ int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_i
 
 int pct_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
-    if ((d_env == nullptr) == (d_mask == nullptr)) { h->err = "pct_reset_envs: pass exactly one of d_env / d_mask"; return PCT_ERR_INVALID; }
-    if (n < 0) { h->err = "pct_reset_envs: n must be >= 0"; return PCT_ERR_INVALID; }
-    if (d_mask && n != h->n_envs) { h->err = "pct_reset_envs: a mask has n_envs entries (n = " + std::to_string(n) + ")"; return PCT_ERR_INVALID; }
-    if (!h->did_reset) { h->err = "pct_reset_envs before pct_reset"; return PCT_ERR_STATE; }
-    if (n == 0) return PCT_OK;
+    const int rc = check_selection(h, "pct_reset_envs", d_env, n, d_mask);
+    if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs) { h->err = "pct_reset_envs: d_obs is NULL"; return PCT_ERR_INVALID; }
     const ResetParams rp{d_env, n, d_mask};
     return launch_pre(h, PreKernel{nullptr, &rp}, d_obs, d_info, (cudaStream_t)stream);

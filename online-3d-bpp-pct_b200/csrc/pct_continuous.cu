@@ -196,11 +196,13 @@ __device__ __noinline__ int genems_warp_c(CEnv *ev, const int n0, const double l
 // ALIAS variant (the default; PCT_B200_ALIAS=0 selects the snapshot kernels): the reference's object semantics of the load entries (EdgePoolA,
 // DESIGN.md section 3 (b)); per-env state through CParams::aux.
 
-template <bool STAB, bool ALIAS = false>
-__global__ void __launch_bounds__(64) pctc_apply_kernel(const CParams p) {
+// SEL: the selected launch (EnvSel, pct_kernels.h)
+template <bool STAB, bool ALIAS = false, bool SEL = false>
+__global__ void __launch_bounds__(64) pctc_apply_kernel(const ParamsT<CParams, SEL> p) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int e = blockIdx.x * 2 + warp;
-    if (e >= p.n_envs) return;
+    int e = blockIdx.x * 2 + warp;
+    if constexpr (SEL) e = sel_env(p.sel, p.n_envs, e);
+    if (e >= p.n_envs || (SEL && e < 0)) return;
     __shared__ int lock_s[2];
     __shared__ __align__(16) double ems_stage[2][CE_STAGE][6];
     int *lock = &lock_s[warp];
@@ -339,12 +341,18 @@ __global__ void __launch_bounds__(64) pctc_apply_kernel(const CParams p) {
 
 // ================= K2: candidates in CPython-set order (C:space.py:531-568) =================
 
-__global__ void __launch_bounds__(32) pctc_candidates_kernel(const CParams p) {
+template <bool SEL = false>
+__global__ void __launch_bounds__(32) pctc_candidates_kernel(const ParamsT<CParams, SEL> p) {
     __shared__ uint32_t tabA[CC_TAB], tabB[512];
     __shared__ uint64_t stg_h[32], rs_h[32];  // staged (hash, code) of the chunk's new keys / of the slots being re-inserted by a resize
     __shared__ uint32_t rs_c[32];
     __shared__ uint16_t stg_c[32];
-    const int lane = threadIdx.x, e = blockIdx.x;
+    const int lane = threadIdx.x;
+    int e = blockIdx.x;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;
+    }
     CEnv *ev = p.env + e;
     int fl = 0;
     if (p.ready) {  // overlapped mode: wait for the apply kernel's hand-over of THIS env
@@ -470,18 +478,21 @@ __global__ void __launch_bounds__(32 * LIGHT_WARPS, 4) pctc_walk_light_kernel(co
 __global__ void __launch_bounds__(32 * WALK_WARPS, 8) pctc_walk_kernel(const CParams p) { PCT_WALK_CONT_BODY(CWalk, p) }
 __global__ void __launch_bounds__(32 * WALK_WARPS, 8) pctc_walk_fork_kernel(const CParams p) { walk_fork<CWalk>(p); }
 
-template <typename OT> __device__ __noinline__ void write_obs_c_delta(const CParams &p, int e, const CEnv *ev, const double (*leaf)[6], int n_leaf, int tid, int nthreads);
+template <typename OT, bool SEL = false> __device__ __noinline__ void write_obs_c_delta(const CParams &p, int e, const CEnv *ev, const double (*leaf)[6], int n_leaf, int tid, int nthreads);
 
-// emit (round 2): the first `nl` set feasibility bits in candidate order -> leaf rows, observation; 64 threads per env
-template <typename OT>
-__global__ void __launch_bounds__(64) pctc_emit_kernel(const CParams p) {
+// emit (round 2): the first `nl` set feasibility bits in candidate order -> leaf rows, observation; 64 threads per env.
+// SEL: the selected launch; block 0 empties the pools whether or not its slot holds an env
+template <typename OT, bool SEL = false>
+__global__ void __launch_bounds__(64) pctc_emit_kernel(const ParamsT<CParams, SEL> p) {
     __shared__ double leaf[NL_MAX][6];
     __shared__ int s_nleaf;
-    const int tid = threadIdx.x, lane = tid & 31, e = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31, e = slot_env<SEL>(p, blockIdx.x);
+    if (SEL && blockIdx.x == 0 && tid == 0) reset_walk_pools(p.walk);
+    if (SEL && e < 0) return;  // the whole block
     CEnv *ev = p.env + e;
     const CHdr &h = ev->h;
     const double nb[3] = {h.next_box[0], h.next_box[1], h.next_box[2]};
-    if (e == 0 && tid == 0) reset_walk_pools(p.walk);
+    if (!SEL && e == 0 && tid == 0) reset_walk_pools(p.walk);
     if (tid == 0) wait_walks(&ev->n_pending, ev);
     __syncthreads();
     if (tid < 32) {
@@ -512,7 +523,9 @@ __global__ void __launch_bounds__(64) pctc_emit_kernel(const CParams p) {
             p.info[e].n_leaf = n_leaf; p.info[e].n_cand = h.n_cand; p.info[e].n_ems = h.n_ems; p.info[e].flags |= h.flags;
         }
     }
-    if (p.delta) write_obs_c_delta<OT>(p, e, ev, leaf, n_leaf, tid, 64);
+    // one instance of the delta writer per kernel: with the whole-batch kernel as its only caller, the compiler specialises the call on that
+    // kernel's `leaf` array, and a shared instance would change the whole-batch kernel's code
+    if (p.delta) write_obs_c_delta<OT, SEL>(p, e, ev, leaf, n_leaf, tid, 64);
     else write_obs_c<OT>(p, e, ev, leaf, n_leaf, tid, 64);
 }
 
@@ -520,7 +533,7 @@ __global__ void __launch_bounds__(64) pctc_emit_kernel(const CParams p) {
 // ================= K3: feasibility per candidate + leaf compaction + observation =================
 // Delta variant of write_obs_c (cf. write_obs_delta, pct_discrete.cu): the caller hands back the same observation buffer, obs_prev[0] / [1] say how
 // many internal / leaf rows of it may be non-zero; only the rows below max(now, prev) and the item row are written.  Same values as write_obs_c.
-template <typename OT>
+template <typename OT, bool SEL>
 __device__ __noinline__ void write_obs_c_delta(const CParams &p, int e, const CEnv *ev, const double (*leaf)[6], int n_leaf, int tid, int nthreads) {
     OT *obs = (OT *)p.obs + (size_t)e * (size_t)((p.nb + p.nl + 1) * 9);
     int32_t *prev = p.aux[e].obs_prev;
@@ -574,13 +587,18 @@ __device__ __forceinline__ double (*rb_store())[5] {  // the default instantiati
 }
 
 // PRE: resting heights from pre-rounded box rectangles staged in shared memory (rest_height_pre; opt-in, PCT_B200_CONT_PRE=1)
-template <typename OT, bool STAB, bool PRE>
-__global__ void __launch_bounds__(64) pctc_feas_emit_kernel(const CParams p) {
+template <typename OT, bool STAB, bool PRE, bool SEL = false>
+__global__ void __launch_bounds__(64) pctc_feas_emit_kernel(const ParamsT<CParams, SEL> p) {
     __shared__ double leaf[NL_MAX][6];
     double (*rb)[5] = rb_store<PRE>();
     __shared__ uint32_t wb[2];
     __shared__ int lock;
-    const int tid = threadIdx.x, lane = tid & 31, e = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31;
+    int e = blockIdx.x;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;  // the whole block
+    }
     CEnv *ev = p.env + e;
     const CHdr &h = ev->h;
     if (tid == 0) {
@@ -648,7 +666,9 @@ __global__ void __launch_bounds__(256) pctc_preview_kernel(const CParams p, cons
     o[0] = h.next_box[0]; o[1] = h.next_box[1]; o[2] = h.next_box[2]; o[3] = h.next_den;
 }
 
-// stands in for pctc_apply_kernel: thread t writes item t (t < n) and initialises env t's info record (t < n_envs)
+// stands in for pctc_apply_kernel: thread t writes item t (t < n) and initialises env t's info record (t < n_envs).
+// SEL (pct_set_items_only): thread t writes item t and the info record of its env, nothing else.
+template <bool SEL = false>
 __global__ void __launch_bounds__(256) pctc_set_items_kernel(const CParams p, const ItemParams ip) {
     const int t = blockIdx.x * 256 + threadIdx.x;
     if (t < ip.n) {
@@ -658,9 +678,15 @@ __global__ void __launch_bounds__(256) pctc_set_items_kernel(const CParams p, co
             CHdr &h = p.env[e].h;
             h.next_box[0] = it[0]; h.next_box[1] = it[1]; h.next_box[2] = it[2];
             if (ip.density) h.next_den = ip.density[t];
+            if (SEL && p.info) {
+                pct_step_info info{};
+                info.counter = h.n_box;
+                info.flags = h.flags;
+                p.info[e] = info;
+            }
         }
     }
-    if (t < p.n_envs && p.info) {
+    if (!SEL && t < p.n_envs && p.info) {
         const CHdr &h = p.env[t].h;
         pct_step_info info{};
         info.counter = h.n_box;
@@ -669,13 +695,23 @@ __global__ void __launch_bounds__(256) pctc_set_items_kernel(const CParams p, co
     }
 }
 
-// stands in for pctc_apply_kernel (pct_reset_envs): warp w resets env w with reset_space_c if selected, then writes its info record
+// stands in for pctc_apply_kernel (pct_reset_envs): warp w resets env w with reset_space_c if selected, then writes its info record.
+// SEL (pct_reset_envs_only): warp w owns slot w of the selection, O(n); unselected envs are not touched.
+template <bool SEL = false>
 __global__ void __launch_bounds__(256) pctc_reset_envs_kernel(const CParams p, const ResetParams rp) {
-    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (e >= p.n_envs) return;  // the whole warp
-    bool sel = rp.mask && rp.mask[e] != 0;
-    if (!rp.mask)
-        for (int i0 = 0; i0 < rp.n && !sel; i0 += 32) sel = __any_sync(FULL, i0 + lane < rp.n && rp.env[i0 + lane] == e);
+    const int w = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    int e = w;
+    bool sel;
+    if constexpr (SEL) {
+        e = sel_env(EnvSel{rp.env, rp.mask, rp.n}, p.n_envs, w);
+        if (e < 0) return;  // the whole warp
+        sel = true;
+    } else {
+        if (e >= p.n_envs) return;  // the whole warp
+        sel = rp.mask && rp.mask[e] != 0;
+        if (!rp.mask)
+            for (int i0 = 0; i0 < rp.n && !sel; i0 += 32) sel = __any_sync(FULL, i0 + lane < rp.n && rp.env[i0 + lane] == e);
+    }
     CEnv *ev = p.env + e;
     if (sel) reset_space_c(ev, p, e, lane);
     if (lane == 0 && p.info) {
@@ -690,13 +726,17 @@ __global__ void __launch_bounds__(256) pctc_reset_envs_kernel(const CParams p, c
 // number of kernels one reset / step enqueues (for pct_kernel_launches): apply, candidates, [light, walk], emit; round 1's kernels: apply, candidates, feas_emit
 int continuous_kernels_per_step(const CParams &p) { return p.walk.walkq && p.setting != 2 ? 5 : 3; }
 
-cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply) {
+// SEL: the selected launch of p.sel (p.ready = nullptr): the SEL instantiations over p.sel.slots(n_envs) slots, the walk kernels as they are
+template <bool SEL>
+static cudaError_t launch_c(const ParamsT<CParams, SEL> &p, int opt, cudaStream_t st, bool apply) {
     const bool stab = p.setting != 2;
-    const int b2 = (p.n_envs + 1) / 2;
+    int slots = p.n_envs;
+    if constexpr (SEL) slots = p.sel.slots(p.n_envs);
+    const int b2 = (slots + 1) / 2;
     if (apply) {
-        if (stab && (opt & PCT_OPT_ALIAS)) pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);
-        else if (stab) pctc_apply_kernel<true><<<b2, 64, 0, st>>>(p);
-        else pctc_apply_kernel<false><<<b2, 64, 0, st>>>(p);
+        if (stab && (opt & PCT_OPT_ALIAS)) pctc_apply_kernel<true, true, SEL><<<b2, 64, 0, st>>>(p);
+        else if (stab) pctc_apply_kernel<true, false, SEL><<<b2, 64, 0, st>>>(p);
+        else pctc_apply_kernel<false, false, SEL><<<b2, 64, 0, st>>>(p);
     }
     // candidates / feas_emit: with p.ready as programmatic dependent launches (their blocks become resident during the previous
     // kernel's tail and wait per env on the hand-over flags), else plain back-to-back launches
@@ -707,48 +747,60 @@ cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool a
     cfg.stream = st; cfg.attrs = at; cfg.numAttrs = p.ready ? 1 : 0;
     // delta observation rows (emit kernel): a buffer other than the tracked one may hold anything -> "all rows"
     if (opt & PCT_OPT_FILL_PREV) launch_fill_prev(p.aux, p.n_envs, p.nb, p.nl, st);
-    cfg.gridDim = dim3(p.n_envs); cfg.blockDim = dim3(32);
-    cudaLaunchKernelEx(&cfg, pctc_candidates_kernel, p);
+    cfg.gridDim = dim3(slots); cfg.blockDim = dim3(32);
+    cudaLaunchKernelEx(&cfg, pctc_candidates_kernel<SEL>, p);
     if (p.walk.walkq) {
         if (stab) {
             int n_sm = 0;
             const cudaError_t es = sm_count(&n_sm);
             if (es != cudaSuccess) return es;
-            pctc_walk_light_kernel<<<n_sm * 4, 32 * LIGHT_WARPS, 0, st>>>(p);
-            if (p.walk.walk_fork) pctc_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, 8)), 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
-            else pctc_walk_kernel<<<n_sm * 8, 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
+            const CParams &pw = p;  // the walks carry their env and size the continuation pool from p.n_envs: the same kernels serve a selection
+            pctc_walk_light_kernel<<<n_sm * 4, 32 * LIGHT_WARPS, 0, st>>>(pw);
+            if (p.walk.walk_fork) pctc_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, 8)), 32 * WALK_WARPS, 0, st>>>(pw);  // one resident wave
+            else pctc_walk_kernel<<<n_sm * 8, 32 * WALK_WARPS, 0, st>>>(pw);  // one resident wave
         }
         cudaLaunchConfig_t c2{};
         c2.stream = st; c2.attrs = at; c2.numAttrs = (stab && !(opt & PCT_OPT_NO_EMIT_PDL)) ? 1 : 0;
-        c2.gridDim = dim3(p.n_envs); c2.blockDim = dim3(64);
-        if (p.obs_f64) cudaLaunchKernelEx(&c2, pctc_emit_kernel<double>, p);
-        else cudaLaunchKernelEx(&c2, pctc_emit_kernel<float>, p);
+        c2.gridDim = dim3(slots); c2.blockDim = dim3(64);
+        if (p.obs_f64) cudaLaunchKernelEx(&c2, pctc_emit_kernel<double, SEL>, p);
+        else cudaLaunchKernelEx(&c2, pctc_emit_kernel<float, SEL>, p);
         return cudaGetLastError();
     }
     cfg.blockDim = dim3(64);
     if (opt & PCT_OPT_CONT_PRE) {
-        if (p.obs_f64) { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, true, true>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, false, true>, p); }
-        else { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, true, true>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, false, true>, p); }
+        if (p.obs_f64) { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, true, true, SEL>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, false, true, SEL>, p); }
+        else { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, true, true, SEL>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, false, true, SEL>, p); }
     } else {
-        if (p.obs_f64) { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, true, false>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, false, false>, p); }
-        else { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, true, false>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, false, false>, p); }
+        if (p.obs_f64) { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, true, false, SEL>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<double, false, false, SEL>, p); }
+        else { if (stab) cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, true, false, SEL>, p); else cudaLaunchKernelEx(&cfg, pctc_feas_emit_kernel<float, false, false, SEL>, p); }
     }
     return cudaGetLastError();
 }
 
-cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st) {
-    const int n = max(ip.n, p.n_envs);
-    pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, ip);
-    cudaError_t err = cudaGetLastError();
-    if (err != cudaSuccess) return err;
-    return launch_continuous(p, opt, st, false);
+cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply, const EnvSel *sel) {
+    if (!sel) return launch_c<false>(p, opt, st, apply);
+    SelParams<CParams> ps;
+    static_cast<CParams &>(ps) = p;
+    ps.sel = *sel;
+    return launch_c<true>(ps, opt, st, apply);
 }
 
-cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st) {
-    pctc_reset_envs_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, rp);
+cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st, const EnvSel *sel) {
+    const int n = sel ? ip.n : max(ip.n, p.n_envs);
+    if (sel) pctc_set_items_kernel<true><<<(n + 255) / 256, 256, 0, st>>>(p, ip);
+    else pctc_set_items_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, ip);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;
-    return launch_continuous(p, opt, st, false);
+    return launch_continuous(p, opt, st, false, sel);
+}
+
+cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
+    const int slots = sel ? sel->slots(p.n_envs) : p.n_envs;
+    if (sel) pctc_reset_envs_kernel<true><<<(slots + 7) / 8, 256, 0, st>>>(p, rp);
+    else pctc_reset_envs_kernel<<<(slots + 7) / 8, 256, 0, st>>>(p, rp);
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    return launch_continuous(p, opt, st, false, sel);
 }
 
 cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st) {

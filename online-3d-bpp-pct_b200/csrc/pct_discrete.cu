@@ -306,13 +306,20 @@ __device__ __forceinline__ void order_file(int32_t *ord, int n_envs, int e, int 
 constexpr int K1_SM_PER_WARP = sizeof(DEnvHot) + EMS_TMP_MAX * 12 + 16 + EDGE_STAGE * 32 + POLY_STAGE * 16 + EMS_TMP_MAX * 8;  // record + EMS temp + mbarrier/lock + staged loads + packed EMS temp
 static_assert(K1_SM_PER_WARP % 16 == 0, "alignment");
 
-template <bool STAB, bool ALIAS = false>
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kernel(const __grid_constant__ DParams p) {  // ALIAS: see EdgePoolA (the default; PCT_B200_ALIAS=0 selects the snapshot kernel)
+// SEL: the selected launch (EnvSel): slot -> the selection's env, no scheduling order
+template <bool STAB, bool ALIAS = false, bool SEL = false>
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kernel(const __grid_constant__ ParamsT<DParams, SEL> p) {  // ALIAS: see EdgePoolA (the default; PCT_B200_ALIAS=0 selects the snapshot kernel)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slot = blockIdx.x * WARPS_PER_BLOCK + warp;
-    if (slot >= p.n_envs) return;
-    const int e = (p.order && p.mode == 1) ? order_lookup(p.order, p.n_envs, slot, lane) : slot;  // heaviest envs first (longest-processing-time-first)
+    int e;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, slot);
+        if (e < 0) return;
+    } else {
+        if (slot >= p.n_envs) return;
+        e = (p.order && p.mode == 1) ? order_lookup(p.order, p.n_envs, slot, lane) : slot;  // heaviest envs first (longest-processing-time-first)
+    }
     unsigned char *sm = smem_raw + (size_t)warp * K1_SM_PER_WARP;
     DEnvHot *hot = (DEnvHot *)sm;
     // per-warp layout: record | EMS temp (3 KB) | packed EMS temp (2 KB) | mbarrier + lock | staged loads | staged polygons.  The two EMS areas are
@@ -533,14 +540,20 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kerne
 // ---- K2: candidate leaves -----------------------------------------------------------------------------------
 // __grid_constant__ (K1, K2, emit): the __noinline__ phases take `const DParams &`; without it every thread first copies the 320 B parameter
 // block into its local-memory frame, so that the reference has an address, and reads the fields back from there.
-template <typename SlotT, bool BIGSM>
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K2_MINB) pct_candidates_kernel(const __grid_constant__ DParams p) {
+template <typename SlotT, bool BIGSM, bool SEL = false>
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K2_MINB) pct_candidates_kernel(const __grid_constant__ ParamsT<DParams, SEL> p) {
     typedef Lay<SlotT, BIGSM> LY;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slot = blockIdx.x * WARPS_PER_BLOCK + warp;
-    if (slot >= p.n_envs) return;
-    const int e = (p.order && p.mode == 1) ? order_lookup(p.order, p.n_envs, slot, lane) : slot;
+    int e;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, slot);
+        if (e < 0) return;
+    } else {
+        if (slot >= p.n_envs) return;
+        e = (p.order && p.mode == 1) ? order_lookup(p.order, p.n_envs, slot, lane) : slot;
+    }
     unsigned char *sm = smem_raw + (size_t)warp * LY::PER_WARP;
     DEnvHot *hot = (DEnvHot *)(sm + LY::HOT);
     SlotT *tabA = (SlotT *)(sm + LY::TAB_A_OFF), *tabB = (SlotT *)(sm + LY::TAB_B_OFF);
@@ -678,12 +691,16 @@ struct FeasSmD {
     uint32_t wb[FEAS_WARPS];
 };
 
-template <typename OT, bool STAB, typename SlotT, bool DELTA = false>
-__global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(const DParams p) {
+template <typename OT, bool STAB, typename SlotT, bool DELTA = false, bool SEL = false>
+__global__ void __launch_bounds__(FEAS_THREADS, K3_MINB) pct_feas_emit_kernel(const ParamsT<DParams, SEL> p) {
     constexpr int BITS = sizeof(SlotT) == 2 ? 4 : 8;
     __shared__ __align__(16) FeasSmD sm;
     const int tid = threadIdx.x, lane = tid & 31;
-    const int e = blockIdx.x;  // (round 1's heaviest-first permutation of this kernel went with the sorting pass; the legacy mode runs in env order)
+    int e = blockIdx.x;  // (round 1's heaviest-first permutation of this kernel went with the sorting pass; the legacy mode runs in env order)
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;  // the whole block
+    }
     DEnvHot *hot = &sm.s.hot;
     DEnvHot *ghot = p.hot + e;
     DEnvCold *cold = p.cold + e;
@@ -810,12 +827,12 @@ constexpr int EMIT_STAGE = sizeof(DHdr) + NB_MAX * 12;  // header + placed boxes
 constexpr int EMIT_SM_PER_WARP = EMIT_STAGE + NL_MAX * 12 + 48;
 static_assert(EMIT_STAGE % 16 == 0 && EMIT_SM_PER_WARP % 16 == 0, "TMA bulk copies move multiples of 16 bytes");
 
-template <typename OT, typename SlotT, bool DELTA>
-__global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const __grid_constant__ DParams p) {
+template <typename OT, typename SlotT, bool DELTA, bool SEL = false>
+__global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const __grid_constant__ ParamsT<DParams, SEL> p) {
     constexpr int BITS = sizeof(SlotT) == 2 ? 4 : 8;
     __shared__ __align__(16) unsigned char smem[EMIT_WARPS * EMIT_SM_PER_WARP];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int e = blockIdx.x * EMIT_WARPS + warp;
+    int e = blockIdx.x * EMIT_WARPS + warp;
     // last kernel of the launch sequence that touches the walk pools (both walk kernels have completed: plain stream order): empty them for the next step
     if (blockIdx.x == 0 && threadIdx.x == 0 && p.walk.walk_ctr) reset_walk_pools(p.walk);
     if (blockIdx.x == 0 && p.order) {
@@ -825,6 +842,10 @@ __global__ void __launch_bounds__(32 * EMIT_WARPS) pct_emit_kernel(const __grid_
         if (threadIdx.x < ORD_BUCKETS) p.order[ORD_CNT + ORD_BUCKETS * par + threadIdx.x] = 0;
         __syncthreads();
         if (threadIdx.x == 0) { __threadfence(); *(volatile int32_t *)p.order = par ^ 1; }
+    }
+    if constexpr (SEL) {  // after the pool reset above: block 0 exists whenever the launch does
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;
     }
     if (e >= p.n_envs) return;
     unsigned char *sm = smem + warp * EMIT_SM_PER_WARP;
@@ -912,32 +933,35 @@ static cudaError_t set_smem(K kernel, size_t smem) {
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 }
 
-// apply = false: the pipeline without K1 (pct_set_items / pct_reset_envs: their kernel in pct_items.cu has already run); the caller passes ready = order = nullptr
-template <typename OT, bool STAB, typename SlotT>
-static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
+// apply = false: the pipeline without K1 (pct_set_items / pct_reset_envs: their kernel in pct_items.cu has already run); the caller passes ready = order = nullptr.
+// SEL: the selected launch of p.sel (ready = order = nullptr too): the SEL instantiations over p.sel.slots(n_envs) slots, the walk kernels as they are
+template <typename OT, bool STAB, typename SlotT, bool SEL>
+static cudaError_t launch_t(const ParamsT<DParams, SEL> &p_in, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
     constexpr bool BIGSM = !STAB;
     static bool attr_set = false;
     const size_t smem1 = (size_t)K1_SM_PER_WARP * WARPS_PER_BLOCK;
     const size_t smem2 = (size_t)Lay<SlotT, BIGSM>::PER_WARP * WARPS_PER_BLOCK;
-    DParams p = p_in;
+    ParamsT<DParams, SEL> p = p_in;
     const bool k3_old = (p.opt & PCT_OPT_K3_BLOCK) != 0 || !p.walk.walkq;  // PCT_B200_K3=block: round 1's block-per-env / thread-per-candidate kernel (A/B measurements)
     if (k3_old) p.walk.walkq = nullptr;  // K2 then skips the classification
     if (!attr_set) {
-        cudaError_t err = set_smem(pct_apply_kernel<STAB>, smem1);
-        if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB>, smem1);  // the ALIAS variant (stability settings only)
-        if (err == cudaSuccess) err = set_smem(pct_candidates_kernel<SlotT, BIGSM>, smem2);
+        cudaError_t err = set_smem(pct_apply_kernel<STAB, false, SEL>, smem1);
+        if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB, SEL>, smem1);  // the ALIAS variant (stability settings only)
+        if (err == cudaSuccess) err = set_smem(pct_candidates_kernel<SlotT, BIGSM, SEL>, smem2);
         if (err != cudaSuccess) return err;
         attr_set = true;
     }
-    const int blocks = (p.n_envs + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+    int slots = p.n_envs;
+    if constexpr (SEL) slots = p.sel.slots(p.n_envs);
+    const int blocks = (slots + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
     if (prof) cudaEventRecord(prof[0], st);
     if (apply) {
-        if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
-        else pct_apply_kernel<STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+        if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+        else pct_apply_kernel<STAB, false, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
     }
     if (prof) cudaEventRecord(prof[1], st);
     cudaError_t err = cudaSuccess;
-    if (p.ready) {
+    if (!SEL && p.ready) {
         // overlapped mode (programmatic dependent launch): the candidates blocks become resident while the apply kernel's tail is
         // still running and pick their env up through the per-env hand-over flags
         cudaLaunchAttribute at[1];
@@ -946,20 +970,20 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
         cudaLaunchConfig_t cfg{};
         cfg.stream = st; cfg.attrs = at; cfg.numAttrs = 1;
         cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(32 * WARPS_PER_BLOCK); cfg.dynamicSmemBytes = smem2;
-        err = cudaLaunchKernelEx(&cfg, pct_candidates_kernel<SlotT, BIGSM>, p);
+        err = cudaLaunchKernelEx(&cfg, pct_candidates_kernel<SlotT, BIGSM, SEL>, p);
         if (err != cudaSuccess) return err;
         if (k3_old) {
             cfg.gridDim = dim3(p.n_envs); cfg.blockDim = dim3(FEAS_THREADS); cfg.dynamicSmemBytes = 0;
-            err = (p.opt & PCT_OPT_DELTA) ? cudaLaunchKernelEx(&cfg, pct_feas_emit_kernel<OT, STAB, SlotT, true>, p)
-                             : cudaLaunchKernelEx(&cfg, pct_feas_emit_kernel<OT, STAB, SlotT>, p);
+            err = (p.opt & PCT_OPT_DELTA) ? cudaLaunchKernelEx(&cfg, pct_feas_emit_kernel<OT, STAB, SlotT, true, SEL>, p)
+                             : cudaLaunchKernelEx(&cfg, pct_feas_emit_kernel<OT, STAB, SlotT, false, SEL>, p);
             if (err != cudaSuccess) return err;
         }
     } else {
-        pct_candidates_kernel<SlotT, BIGSM><<<blocks, 32 * WARPS_PER_BLOCK, smem2, st>>>(p);
+        pct_candidates_kernel<SlotT, BIGSM, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem2, st>>>(p);
         if (prof) cudaEventRecord(prof[2], st);
         if (k3_old) {
-            if (p.opt & PCT_OPT_DELTA) pct_feas_emit_kernel<OT, STAB, SlotT, true><<<p.n_envs, FEAS_THREADS, 0, st>>>(p);
-            else pct_feas_emit_kernel<OT, STAB, SlotT><<<p.n_envs, FEAS_THREADS, 0, st>>>(p);
+            if (p.opt & PCT_OPT_DELTA) pct_feas_emit_kernel<OT, STAB, SlotT, true, SEL><<<slots, FEAS_THREADS, 0, st>>>(p);
+            else pct_feas_emit_kernel<OT, STAB, SlotT, false, SEL><<<slots, FEAS_THREADS, 0, st>>>(p);
         }
     }
     if (!k3_old) {
@@ -969,11 +993,12 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
             int n_sm = 0;
             err = sm_count(&n_sm);
             if (err != cudaSuccess) return err;
-            pct_walk_light_kernel<<<n_sm * LIGHT_MINB, 32 * LIGHT_WARPS, 0, st>>>(p);
-            if (p.walk.walk_fork) pct_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, WALK_MINB)), 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave
-            else pct_walk_kernel<<<n_sm * WALK_MINB, 32 * WALK_WARPS, 0, st>>>(p);  // one resident wave (every block starts at once: the emit kernel may follow)
+            const DParams &pw = p;  // the walks carry their env (WalkItem::env) and size the continuation pool from p.n_envs: the same kernels serve a selection
+            pct_walk_light_kernel<<<n_sm * LIGHT_MINB, 32 * LIGHT_WARPS, 0, st>>>(pw);
+            if (p.walk.walk_fork) pct_walk_fork_kernel<<<n_sm * max(1, min(p.walk.walk_blocks, WALK_MINB)), 32 * WALK_WARPS, 0, st>>>(pw);  // one resident wave
+            else pct_walk_kernel<<<n_sm * WALK_MINB, 32 * WALK_WARPS, 0, st>>>(pw);  // one resident wave (every block starts at once: the emit kernel may follow)
         }
-        const int eb = (p.n_envs + EMIT_WARPS - 1) / EMIT_WARPS;
+        const int eb = (slots + EMIT_WARPS - 1) / EMIT_WARPS;
         {   // programmatic dependent of the continuation kernel (setting 2: of the candidates kernel, whose blocks never trigger early -> plain order)
             cudaLaunchAttribute at[1];
             at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -981,7 +1006,7 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
             cudaLaunchConfig_t cfg{};
             cfg.stream = st; cfg.attrs = at; cfg.numAttrs = (STAB && p.ready && !(p.opt & PCT_OPT_NO_EMIT_PDL)) ? 1 : 0;
             cfg.gridDim = dim3(eb); cfg.blockDim = dim3(32 * EMIT_WARPS); cfg.dynamicSmemBytes = 0;
-            err = (p.opt & PCT_OPT_DELTA) ? cudaLaunchKernelEx(&cfg, pct_emit_kernel<OT, SlotT, true>, p) : cudaLaunchKernelEx(&cfg, pct_emit_kernel<OT, SlotT, false>, p);
+            err = (p.opt & PCT_OPT_DELTA) ? cudaLaunchKernelEx(&cfg, pct_emit_kernel<OT, SlotT, true, SEL>, p) : cudaLaunchKernelEx(&cfg, pct_emit_kernel<OT, SlotT, false, SEL>, p);
             if (err != cudaSuccess) return err;
         }
     }
@@ -989,9 +1014,16 @@ static cudaError_t launch_t(const DParams &p_in, cudaStream_t st, cudaEvent_t *p
     return cudaGetLastError();
 }
 template <typename OT, bool STAB>
-static cudaError_t launch_s(const DParams &p, cudaStream_t st, cudaEvent_t *prof, bool apply = true) {
-    if (p.W <= 16 && p.L <= 16 && p.H <= 16) return launch_t<OT, STAB, uint16_t>(p, st, prof, apply);
-    return launch_t<OT, STAB, uint32_t>(p, st, prof, apply);
+static cudaError_t launch_s(const DParams &p, cudaStream_t st, cudaEvent_t *prof, bool apply, const EnvSel *sel) {
+    const bool narrow = p.W <= 16 && p.L <= 16 && p.H <= 16;
+    if (sel) {
+        SelParams<DParams> ps;
+        static_cast<DParams &>(ps) = p;
+        ps.sel = *sel;
+        return narrow ? launch_t<OT, STAB, uint16_t, true>(ps, st, nullptr, apply) : launch_t<OT, STAB, uint32_t, true>(ps, st, nullptr, apply);
+    }
+    if (narrow) return launch_t<OT, STAB, uint16_t, false>(p, st, prof, apply);
+    return launch_t<OT, STAB, uint32_t, false>(p, st, prof, apply);
 }
 
 // number of kernels one reset / step enqueues (for pct_kernel_launches): apply, candidates (+ classify), [walk], emit, order / pool reset
@@ -1000,10 +1032,10 @@ int discrete_kernels_per_step(const DParams &p) {
     return 3 + (p.setting != 2 ? 2 : 0);
 }
 
-cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof, bool apply) {
+cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof, bool apply, const EnvSel *sel) {
     const bool stab = p.setting != 2;
-    if (p.obs_f64) return stab ? launch_s<double, true>(p, st, prof, apply) : launch_s<double, false>(p, st, prof, apply);
-    return stab ? launch_s<float, true>(p, st, prof, apply) : launch_s<float, false>(p, st, prof, apply);
+    if (p.obs_f64) return stab ? launch_s<double, true>(p, st, prof, apply, sel) : launch_s<double, false>(p, st, prof, apply, sel);
+    return stab ? launch_s<float, true>(p, st, prof, apply, sel) : launch_s<float, false>(p, st, prof, apply, sel);
 }
 
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,

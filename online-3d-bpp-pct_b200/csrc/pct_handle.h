@@ -34,6 +34,7 @@ struct pct_env_batch {
     int stream_len = 0;
     int traj_len = 0;
     int32_t *d_ready = nullptr;   // [2 * n_envs] per-env hand-over flags of the overlapped launch mode
+    uint8_t *d_sel_mask = nullptr; // [n_envs] the mask of a selected call, copied before its first kernel (the mask may be a buffer the call writes)
     int32_t epoch = 0;
     bool overlap = true;          // PCT_B200_OVERLAP=0: plain back-to-back kernels
     bool overlap_cont = false;    // continuous domain: measured slower overlapped, off unless PCT_B200_OVERLAP_CONT=1

@@ -5,7 +5,8 @@
 //
 // Override: pct_set_items_kernel stands in for the apply kernel of a step.  It writes the listed envs' next_box / next_den and
 // initialises every env's info record the way the apply kernel does for a successful step (counter, sticky flags, zeros); the
-// rest of the step's pipeline (candidates, walks, emit) then re-expands every env of the batch (launch_discrete with apply = false).
+// rest of the step's pipeline (candidates, walks, emit) then re-expands every env of the batch (launch_discrete with apply = false).  The selected
+// form (pct_set_items_only) writes the listed envs' items and records and re-expands those envs alone.
 //
 // A translation unit of its own (see pct_draw.cuh).
 #include "pct_common.cuh"
@@ -34,7 +35,9 @@ __global__ void __launch_bounds__(ITEM_THREADS) pct_preview_kernel(const DParams
     o[0] = h.next_box[0]; o[1] = h.next_box[1]; o[2] = h.next_box[2]; o[3] = h.next_den;
 }
 
-// thread t: item t of the call (if t < n) and the info record of env t (if t < n_envs); the two never touch the same fields
+// thread t: item t of the call (if t < n) and the info record of env t (if t < n_envs); the two never touch the same fields.
+// SEL (pct_set_items_only): thread t writes item t and the info record of its env, nothing else.
+template <bool SEL = false>
 __global__ void __launch_bounds__(ITEM_THREADS) pct_set_items_kernel(const DParams p, const ItemParams ip) {
     const int t = blockIdx.x * ITEM_THREADS + threadIdx.x;
     if (t < ip.n) {
@@ -45,9 +48,15 @@ __global__ void __launch_bounds__(ITEM_THREADS) pct_set_items_kernel(const DPara
             // a container side is at most 255 (pct_create), the range of the rotation table: a larger side fits nowhere either way
             h.next_box[0] = min(max(it[0], 0), 255); h.next_box[1] = min(max(it[1], 0), 255); h.next_box[2] = min(max(it[2], 0), 255);
             if (ip.density) h.next_den = ip.density[t];
+            if (SEL && p.info) {
+                pct_step_info info{};
+                info.counter = h.n_box;
+                info.flags = h.flags;
+                p.info[e] = info;
+            }
         }
     }
-    if (t < p.n_envs && p.info) {
+    if (!SEL && t < p.n_envs && p.info) {
         const DHdr &h = p.hot[t].h;
         pct_step_info info{};
         info.counter = h.n_box;
@@ -62,12 +71,13 @@ cudaError_t launch_preview_discrete(const DParams &p, const ItemParams &ip, cuda
     return cudaGetLastError();
 }
 
-cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st) {
-    const int n = max(ip.n, p.n_envs);
-    pct_set_items_kernel<<<(n + ITEM_THREADS - 1) / ITEM_THREADS, ITEM_THREADS, 0, st>>>(p, ip);
+cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st, const EnvSel *sel) {
+    const int n = sel ? ip.n : max(ip.n, p.n_envs);
+    if (sel) pct_set_items_kernel<true><<<(n + ITEM_THREADS - 1) / ITEM_THREADS, ITEM_THREADS, 0, st>>>(p, ip);
+    else pct_set_items_kernel<<<(n + ITEM_THREADS - 1) / ITEM_THREADS, ITEM_THREADS, 0, st>>>(p, ip);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;
-    return launch_discrete(p, st, nullptr, false);
+    return launch_discrete(p, st, nullptr, false, sel);
 }
 
 }  // namespace pct

@@ -2,6 +2,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <type_traits>
 #include <cuda_runtime.h>
 #include "pct_b200.h"
 
@@ -241,6 +242,38 @@ static_assert(sizeof(WalkPools<WalkItem>) == 72 && offsetof(DParams, walk) == 24
               "walk pools at the byte offsets of the fields they replaced");
 constexpr int PCT_OPT_DELTA = 1, PCT_OPT_ALIAS = 2, PCT_OPT_K3_BLOCK = 4, PCT_OPT_NO_EMIT_PDL = 8;  // K3_BLOCK: round 1's block-per-env feasibility kernel (A/B)
 
+// The envs of a selected launch (pct_step_envs, pct_reset_envs_only, pct_set_items_only; DESIGN.md section 17).  List form: slot s < n works on
+// env env[s] (env == nullptr: env s); an index outside [0, n_envs) selects nothing.  Mask form (mask non-null, n == n_envs): slot s works on env s
+// iff mask[s] != 0.  The env index is then used exactly as in a whole-batch launch, so an env's trajectory does not depend on the selection.
+struct EnvSel {
+    const int32_t *env;
+    const uint8_t *mask;
+    int32_t n;
+    // grid slots of the launch
+    __host__ __device__ __forceinline__ int slots(int n_envs) const { return mask ? n_envs : n; }
+};
+// env of `slot`, or -1 when the slot works on no env
+__device__ __forceinline__ int sel_env(const EnvSel &s, int n_envs, int slot) {
+    if (slot >= s.slots(n_envs)) return -1;
+    if (s.mask) return s.mask[slot] ? slot : -1;
+    const int e = s.env ? s.env[slot] : slot;
+    return e >= 0 && e < n_envs ? e : -1;
+}
+// Parameters of the selected kernel instantiations (template argument SEL = true): the selection behind an unchanged DParams / CParams, so that no
+// field of the whole-batch kernels (SEL = false: DParams itself) moves.  Every phase keeps taking `const DParams &`.
+template <typename P>
+struct SelParams : P {
+    EnvSel sel;
+};
+template <typename P, bool SEL>
+using ParamsT = typename std::conditional<SEL, SelParams<P>, P>::type;
+// env of grid slot `slot`: the slot itself (whole batch) or the selection's env (-1: none)
+template <bool SEL, typename P>
+__device__ __forceinline__ int slot_env(const P &p, int slot) {
+    if constexpr (SEL) return sel_env(p.sel, p.n_envs, slot);
+    else return slot;
+}
+
 // heuristic baselines (pct_heuristics.cuh)
 struct HParams {
     int code;                // enum pct_heuristic
@@ -282,7 +315,8 @@ struct ItemParams {
 };
 cudaError_t launch_preview_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
 // the item kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
-cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
+// sel non-null: the selected forms (pct_set_items_only / pct_reset_envs_only): only the selected envs are touched
+cudaError_t launch_set_items_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st, const EnvSel *sel = nullptr);
 
 // read-only leaf expansion of caller-given items (pct_expand.cu): row r expands k items on env env[r]
 struct ExpandParams {
@@ -302,7 +336,7 @@ struct ResetParams {
     const uint8_t *mask;     // [n_envs], or nullptr: the env list
 };
 // the reset kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
-cudaError_t launch_reset_envs_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st);
+cudaError_t launch_reset_envs_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel = nullptr);
 
 // the kernel that stands in for the apply kernel of a step, exactly one non-null: the item kernel (pct_set_items) or the reset kernel
 // (pct_reset_envs).  The rest of the step's pipeline then re-expands every env of the batch.
@@ -319,7 +353,8 @@ cudaError_t sm_count(int *n);
 
 int discrete_kernels_per_step(const DParams &p);
 // apply = false: the sequence without the apply kernel (pct_set_items / pct_reset_envs; p.ready and p.order must be nullptr)
-cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof = nullptr, bool apply = true);
+// sel non-null: the selected launch (pct_step_envs; p.ready and p.order must be nullptr): the SEL instantiations over sel->slots(n_envs) slots
+cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof = nullptr, bool apply = true, const EnvSel *sel = nullptr);
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                           cudaStream_t st, const int64_t *t_dev = nullptr);
 
@@ -332,9 +367,10 @@ struct CParams;
 constexpr int PCT_OPT_FILL_PREV = 16, PCT_OPT_CONT_PRE = 32;
 int continuous_kernels_per_step(const CParams &p);
 // apply = false: the sequence without the apply kernel (pct_set_items / pct_reset_envs; p.ready must be nullptr)
-cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply = true);
-cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st);
-cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st);
+// sel: as for the discrete launchers
+cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply = true, const EnvSel *sel = nullptr);
+cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st, const EnvSel *sel = nullptr);
+cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st, const EnvSel *sel = nullptr);
 cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st);
 cudaError_t launch_expand_continuous(const CParams &p, const ExpandParams &x, cudaStream_t st);
 cudaError_t launch_queries_continuous(const CParams &p, const QParams &q, cudaStream_t st);
