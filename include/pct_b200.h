@@ -356,6 +356,51 @@ int pct_reset_envs_only(pct_handle h, const int32_t *d_env, int32_t n, const uin
 int pct_set_items_only(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
                        pct_step_info *d_info, void *stream);
 
+/* Buffered packing ("online packing with buffer"): every env holds B items drawn from its item source, and one step picks the item
+ * and its placement at once, by a flat index into the leaves of all B items (PCT's union of the buffered items' leaf nodes).
+ *
+ * pct_set_buffer turns a handle into a buffered one: call it after pct_create and before the first reset; it allocates the per-env
+ * buffer state (B items, B stored leaf blocks, per-slot expansion scratch).  Errors: PCT_ERR_STATE after a reset; PCT_ERR_INVALID for
+ * B outside [1, 16] and for a handle with no_auto_reset = 1 (gym-style buffered envs are not supported).
+ *
+ * Observation of a buffered handle, pct_buffer_obs_len(h) = (NB + B * NL + B) * 9 values per env, in the handle's obs dtype:
+ *   rows [0, NB)                         the internal-node rows of pct_step, byte for byte;
+ *   rows [NB + j * NL, NB + (j + 1) * NL) leaf block j: the bytes pct_expand_items writes for buffer item j on the env in its current
+ *                                        state (same cast, LNES scheme and keyed shuffle);
+ *   row NB + B * NL + j                  the item row pct_set_items writes for buffer item j.
+ * With B = 1 this is the pct_step layout, and a buffered handle computes what a plain one does.  Every call writes every row (the
+ * delta-row contract of pct_step does not apply).
+ *
+ * pct_buffer_reset: resets every env and fills slots 0 .. B-1 with the env's next B draws in draw order (under
+ * pct_set_trajectory_length: the first B items of the next trajectory); writes the whole observation and, when d_info is given, the
+ * records (n_leaf and n_cand summed over the slots).
+ *
+ * pct_buffer_step: d_leaf_idx[e] = j * NL + l picks leaf l of buffer item j.  The step of env e is exactly pct_set_items(e, item j)
+ * followed by pct_step(leaf_idx = l) on a plain handle: placement, reward, done, BAD_ACTION and capacity flags, the zero action for
+ * l >= the slot's leaf count, and the auto-reset.  An index outside [0, B * NL) acts as slot 0 with leaf index -1.  Then:
+ *   a placed item's slot takes the draw the step consumed, the other slots keep their items;
+ *   a finished episode resets the env and refills the whole buffer as pct_buffer_reset does;
+ *   every slot is expanded against the new state; capacity flags raised by any slot's expansion join the env's sticky flags.
+ * The record: counter, flags, ratio, ep_reward and ep_len as pct_step writes them; n_leaf and n_cand summed over the slots; n_ems.
+ * Leaf rows name no slot, so actions are flat leaf indices only.
+ *
+ * pct_buffer_items: d_out <- n x B x 4 float64 [x, y, z, density] of envs d_env[0..n) (NULL: envs 0..n-1), each slot's item as drawn
+ * (not the sorted sizes of its item row); read-only.  An index outside [0, n_envs) gives zeros.
+ * pct_buffer_policy_random: d_idx[e] <- a uniform valid flat leaf index: the k-th valid leaf of the slots in order, k =
+ * rnd(seed, global env id, *d_t) % (sum of the slots' leaf counts); 0 when no slot has a leaf.  *d_t is read when the kernel runs.
+ *
+ * All of them only enqueue work on `stream` (no host synchronisation, no allocation: CUDA-graph capturable).  On a buffered handle the
+ * read-only calls (pct_query_placements*, pct_height_maps, pct_expand_items, pct_get_state, pct_get_support_graph) see the env's placed
+ * boxes; pct_reset, pct_step, pct_step_envs, the _host calls, pct_set_items*, pct_reset_envs*, pct_preview_items,
+ * pct_heuristic_actions* and pct_snapshot / pct_restore return PCT_ERR_STATE.  The buffered calls return PCT_ERR_STATE on a handle
+ * without pct_set_buffer, and pct_buffer_step / _items / _policy_random before pct_buffer_reset. */
+int pct_set_buffer(pct_handle h, int32_t B);
+int32_t pct_buffer_obs_len(pct_handle h);
+int pct_buffer_reset(pct_handle h, void *d_obs, pct_step_info *d_info, void *stream);
+int pct_buffer_step(pct_handle h, const int32_t *d_leaf_idx, void *d_obs, float *d_reward, uint8_t *d_done, pct_step_info *d_info, void *stream);
+int pct_buffer_items(pct_handle h, const int32_t *d_env, int32_t n, double *d_out, void *stream);
+int pct_buffer_policy_random(pct_handle h, int32_t *d_idx, uint64_t seed, const int64_t *d_t, void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

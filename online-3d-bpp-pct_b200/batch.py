@@ -20,9 +20,12 @@ class PctBatch(object):
     def __init__(self, n_envs, setting, container_size=(10, 10, 10), item_set=None, internal_node_holder=80,
                  leaf_node_holder=50, continuous=False, obs_dtype=torch.float32, seed=0, env_id_base=0, device=0,
                  sample_from_distribution=False, sample_left_bound=None, sample_right_bound=None, item_stream=None,
-                 size_minimum=None, auto_reset=True, LNES="EMS", shuffle=False):
+                 size_minimum=None, auto_reset=True, LNES="EMS", shuffle=False, buffer=None):
         """shuffle: the reference's `shuffle` kwarg (D:bin3D.py:114-115; tools.py:136 defaults --shuffle to True for training): the ordered candidate list
-        is permuted before the feasibility tests and the leaf cap, by a keyed counter-based permutation (include/pct_b200.h, pct_config::shuffle)."""
+        is permuted before the feasibility tests and the leaf cap, by a keyed counter-based permutation (include/pct_b200.h, pct_config::shuffle).
+        buffer=B (1..16): buffered packing (pct_set_buffer): every env holds B items, the observation carries the leaves of all of them
+        ((NB + B * NL + B) rows: internal nodes, B leaf blocks, B item rows; obs_len follows), and step(leaf_idx=j * NL + l) places leaf l of
+        item j; reset / step / random_policy_dev go to the buffered calls and buffer_items() reads the buffered items."""
         if not torch.cuda.is_available():
             raise PctError("pct_b200 needs a CUDA device (sm_90a kernels; there is no CPU fallback)")
         self.L = _lib.lib()
@@ -68,7 +71,12 @@ class PctBatch(object):
         if rc != 0:
             raise PctError("pct_create failed (%d): %s" % (rc, self.L.pct_last_error(None).decode()))
         self.h = h
-        self.obs_len = self.L.pct_obs_len(self.h)
+        self.buffer = None if buffer is None else int(buffer)
+        if self.buffer is not None:
+            self._check(self.L.pct_set_buffer(self.h, self.buffer), "pct_set_buffer")
+            self.obs_len = self.L.pct_buffer_obs_len(self.h)
+        else:
+            self.obs_len = self.L.pct_obs_len(self.h)
         if item_set is not None:
             self.set_item_set(item_set)
         if item_stream is not None:
@@ -137,6 +145,14 @@ class PctBatch(object):
         (n_envs, 8) int32 tensor for the pct_step_info records of the new expansions.  An empty env_idx enqueues nothing.
         whole_batch=False (pct_reset_envs_only): only the chosen envs are re-expanded, and only their rows of `out` and of `info` are
         written, at a cost in proportion to the chosen envs."""
+        if self.buffer is not None and env_idx is None and mask is None:  # pct_buffer_reset: every env, the buffers refilled
+            obs = self._obs if out is None else out
+            if info is not None:
+                info = self._out(info, (self.n_envs, 8), torch.int32, "reset info")
+            self._check(self.L.pct_buffer_reset(self.h, C.c_void_p(obs.data_ptr()), C.c_void_p(info.data_ptr()) if info is not None else None,
+                                                self._stream()), "pct_buffer_reset")
+            self.did_reset = True
+            return obs
         if env_idx is None and mask is None:
             if info is not None:
                 raise PctError("reset: info is written by a reset of chosen envs (env_idx or mask) only")
@@ -165,6 +181,12 @@ class PctBatch(object):
         (pct_step_envs), at a cost in proportion to them.  actions / leaf_idx keep their full size and only the chosen envs' rows are read;
         only the chosen envs' rows of the four returned buffers are written.  An empty env_idx enqueues nothing."""
         sel = env_idx is not None or mask is not None
+        if self.buffer is not None and not sel and actions is None:  # pct_buffer_step: flat leaf indices j * NL + l
+            obs = self._obs if out is None else out
+            leaf_idx = leaf_idx.to(torch.int32).contiguous()
+            self._check(self.L.pct_buffer_step(self.h, C.c_void_p(leaf_idx.data_ptr()), C.c_void_p(obs.data_ptr()), C.c_void_p(self._rew.data_ptr()),
+                                               C.c_void_p(self._done.data_ptr()), C.c_void_p(self._info.data_ptr()), self._stream()), "pct_buffer_step")
+            return obs, self._rew, self._done, self._info
         if sel:
             idx, m, n = self._selection(env_idx, mask, "step")
         obs = self._obs if out is None else out
@@ -199,8 +221,13 @@ class PctBatch(object):
         return idx
 
     def random_policy_dev(self, seed, t_dev, out=None):
-        """random_policy with the step counter read from a device int64 tensor at execution time (graph-capturable)"""
+        """random_policy with the step counter read from a device int64 tensor at execution time (graph-capturable).  Buffered batch:
+        a uniform valid flat leaf index over all buffered items (pct_buffer_policy_random)."""
         idx = self._idx if out is None else out
+        if self.buffer is not None:
+            self._check(self.L.pct_buffer_policy_random(self.h, C.c_void_p(idx.data_ptr()), int(seed) & ((1 << 64) - 1), C.c_void_p(t_dev.data_ptr()),
+                                                        self._stream()), "pct_buffer_policy_random")
+            return idx
         self._check(self.L.pct_policy_random_dev(self.h, C.c_void_p(idx.data_ptr()), int(seed) & ((1 << 64) - 1), C.c_void_p(t_dev.data_ptr()),
                                                  self._stream()), "pct_policy_random_dev")
         return idx
@@ -457,6 +484,20 @@ class PctBatch(object):
         self._check(self.L.pct_expand_items(self.h, ptr(idx), n, k, ptr(it), ptr(den), ptr(leaves), ptr(info), self._stream()),
                     "pct_expand_items")
         return leaves, info
+
+    def buffer_items(self, env_idx=None, out=None):
+        """The buffered items of envs env_idx (default: every env) -> (n, B, 4) float64 CUDA tensor of [x, y, z, density] per slot, as
+        drawn (not the sorted sizes of the item rows); read-only, enqueued on the current stream.  Rows of an index outside [0, n_envs)
+        are zeros.  Buffered batches only."""
+        if self.buffer is None:
+            raise PctError("buffer_items: not a buffered batch (PctBatch(..., buffer=B))")
+        idx = self._index(env_idx, "env_idx")
+        n = self.n_envs if idx is None else int(idx.numel())
+        shape = (n, self.buffer, 4)
+        out = torch.empty(shape, dtype=torch.float64, device=self.device) if out is None else self._out(out, shape, torch.float64, "buffer_items out")
+        self._check(self.L.pct_buffer_items(self.h, C.c_void_p(idx.data_ptr()) if idx is not None and n else None, n,
+                                            C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_buffer_items")
+        return out
 
     # -- host-buffer API (what the reference's VecEnv exchanges over its pipes) --------------------------------
     def reset_host(self, obs_out):

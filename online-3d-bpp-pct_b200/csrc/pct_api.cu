@@ -95,6 +95,13 @@ static bool capturing(cudaStream_t st) {
     return cap != cudaStreamCaptureStatusNone;
 }
 
+// The calls whose state model does not know the buffer of a buffered handle (pct_set_buffer) refuse it
+static int refuse_buffered(pct_handle h, const char *what) {
+    if (!h->buf_B) return PCT_OK;
+    h->err = std::string(what) + ": not on a buffered handle (pct_set_buffer); use the pct_buffer_* calls";
+    return PCT_ERR_STATE;
+}
+
 extern "C" {
 
 const char *pct_version(void) { return "pct_b200 0.1 (sm_90a)"; }
@@ -239,6 +246,7 @@ void pct_destroy(pct_handle h) {
     cudaFree(h->d_hstate); cudaFree(h->d_hstate_c); cudaFree(h->d_query_c); cudaFree(h->d_query); cudaFree(h->d_aux);
     cudaFree(h->d_ready); cudaFree(h->d_sel_mask);
     cudaFree(h->d_hot); cudaFree(h->d_cold); cudaFree(h->d_item_set); cudaFree(h->d_stream);
+    cudaFree(h->d_buf_items); cudaFree(h->d_buf_leaf); cudaFree(h->d_buf_nleaf); cudaFree(h->d_buf_l); cudaFree(h->d_buf_scratch);
     cudaFree(h->d_obs); cudaFree(h->d_act); cudaFree(h->d_idx); cudaFree(h->d_rew); cudaFree(h->d_done); cudaFree(h->d_info);
     for (cudaEvent_t ev : h->prof_ev) if (ev) cudaEventDestroy(ev);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
@@ -398,6 +406,7 @@ static int launch(pct_handle h, int mode, const void *actions, int action_f64, c
 
 int pct_reset(pct_handle h, void *d_obs, void *stream) {
     if (!h || !d_obs) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_reset")) return PCT_ERR_STATE;
     int rc = launch(h, 0, nullptr, 0, nullptr, d_obs, nullptr, nullptr, nullptr, (cudaStream_t)stream);
     if (rc == PCT_OK) h->did_reset = true;
     return rc;
@@ -407,6 +416,7 @@ int pct_step(pct_handle h, const void *d_actions, int32_t action_f64, const int3
              uint8_t *d_done, pct_step_info *d_info, void *stream) {
     if (!h || !d_obs || !d_reward || !d_done) return PCT_ERR_INVALID;
     if ((d_actions == nullptr) == (d_leaf_idx == nullptr)) { h->err = "pct_step: pass exactly one of d_actions / d_leaf_idx"; return PCT_ERR_INVALID; }
+    if (refuse_buffered(h, "pct_step")) return PCT_ERR_STATE;
     if (!h->did_reset) { h->err = "pct_step before pct_reset"; return PCT_ERR_STATE; }
     return launch(h, 1, d_actions, action_f64, d_leaf_idx, d_obs, d_reward, d_done, d_info, (cudaStream_t)stream);
 }
@@ -425,6 +435,7 @@ static int ensure_staging(pct_handle h) {
 
 int pct_reset_host(pct_handle h, void *h_obs) {
     if (!h || !h_obs) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_reset_host")) return PCT_ERR_STATE;
     CK(h, cudaSetDevice(h->device));
     int rc = ensure_staging(h);
     if (rc) return rc;
@@ -440,6 +451,7 @@ int pct_step_host(pct_handle h, const void *h_actions, int32_t action_f64, const
                   uint8_t *h_done, pct_step_info *h_info) {
     if (!h || !h_obs || !h_reward || !h_done) return PCT_ERR_INVALID;
     if ((h_actions == nullptr) == (h_leaf_idx == nullptr)) { h->err = "pct_step_host: pass exactly one of actions / leaf_idx"; return PCT_ERR_INVALID; }
+    if (refuse_buffered(h, "pct_step_host")) return PCT_ERR_STATE;
     if (!h->did_reset) { h->err = "pct_step_host before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
     int rc = ensure_staging(h);
@@ -533,6 +545,7 @@ int pct_policy_random_dev(pct_handle h, int32_t *d_leaf_idx, uint64_t seed, cons
 int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64_t seed, int64_t t, void *stream) {
     if (!h || !d_rows) return PCT_ERR_INVALID;
     if (heuristic < PCT_H_LSAH || heuristic > PCT_H_RANDOM) { h->err = "pct_heuristic_actions: unknown heuristic"; return PCT_ERR_INVALID; }
+    if (refuse_buffered(h, "pct_heuristic_actions")) return PCT_ERR_STATE;
     if (h->cfg.domain != PCT_DISCRETE) { h->err = "pct_heuristic_actions: discrete domain only"; return PCT_ERR_INVALID; }
     if (!h->did_reset) { h->err = "pct_heuristic_actions before pct_reset"; return PCT_ERR_STATE; }
     CK(h, cudaSetDevice(h->device));
@@ -546,6 +559,7 @@ int pct_heuristic_actions(pct_handle h, int32_t heuristic, float *d_rows, uint64
 
 int pct_heuristic_actions_f64(pct_handle h, int32_t heuristic, double *d_rows, void *stream) {
     if (!h || !d_rows) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_heuristic_actions_f64")) return PCT_ERR_STATE;
     if (h->cfg.domain != PCT_CONTINUOUS) { h->err = "pct_heuristic_actions_f64: continuous domain only (discrete: pct_heuristic_actions)"; return PCT_ERR_INVALID; }
     if (heuristic != PCT_H_LSAH && heuristic != PCT_H_ONLINEBPH && heuristic != PCT_H_BR) {  // tools.py:217-218
         h->err = "only LSAH, OnlineBPH, and BR allowed for continuous environment";
@@ -678,6 +692,7 @@ static int check_items(pct_handle h, const char *what, int32_t n, int32_t k, con
 
 int pct_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, double *d_out, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_preview_items")) return PCT_ERR_STATE;
     int rc = check_items(h, "pct_preview_items", n, k, d_out, "d_out");
     if (rc != PCT_OK || n == 0) return rc;
     CK(h, cudaSetDevice(h->device));
@@ -739,6 +754,7 @@ static int resolve_selection(pct_handle h, const int32_t *d_env, int32_t n, cons
 int pct_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, const void *d_actions, int32_t action_f64,
                   const int32_t *d_leaf_idx, void *d_obs, float *d_reward, uint8_t *d_done, pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_step_envs")) return PCT_ERR_STATE;
     int rc = check_selection(h, "pct_step_envs", d_env, n, d_mask);
     if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs || !d_reward || !d_done) { h->err = "pct_step_envs: d_obs, d_reward and d_done must not be NULL"; return PCT_ERR_INVALID; }
@@ -760,6 +776,7 @@ int pct_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *
 
 int pct_reset_envs_only(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_reset_envs_only")) return PCT_ERR_STATE;
     int rc = check_selection(h, "pct_reset_envs_only", d_env, n, d_mask);
     if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs) { h->err = "pct_reset_envs_only: d_obs is NULL"; return PCT_ERR_INVALID; }
@@ -774,6 +791,7 @@ int pct_reset_envs_only(pct_handle h, const int32_t *d_env, int32_t n, const uin
 int pct_set_items_only(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
                        pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_set_items_only")) return PCT_ERR_STATE;
     int rc = check_items(h, "pct_set_items_only", n, 1, d_items, "d_items");
     if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs) { h->err = "pct_set_items_only: d_obs is NULL"; return PCT_ERR_INVALID; }
@@ -785,6 +803,7 @@ int pct_set_items_only(pct_handle h, const int32_t *d_env, int32_t n, const void
 int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_items, const double *d_density, void *d_obs,
                   pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_set_items")) return PCT_ERR_STATE;
     int rc = check_items(h, "pct_set_items", n, 1, d_items, "d_items");
     if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs) { h->err = "pct_set_items: d_obs is NULL"; return PCT_ERR_INVALID; }
@@ -794,6 +813,7 @@ int pct_set_items(pct_handle h, const int32_t *d_env, int32_t n, const void *d_i
 
 int pct_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_reset_envs")) return PCT_ERR_STATE;
     const int rc = check_selection(h, "pct_reset_envs", d_env, n, d_mask);
     if (rc != PCT_OK || n == 0) return rc;
     if (!d_obs) { h->err = "pct_reset_envs: d_obs is NULL"; return PCT_ERR_INVALID; }
@@ -875,10 +895,121 @@ int pct_get_support_graph(pct_handle h, int32_t env, pct_support_graph *out) {
     return PCT_OK;
 }
 
+// ---- buffered packing (pct_buffer.cu) ----
+static BufParams buffer_params(const pct_env_batch *h) {
+    BufParams b{};
+    b.B = h->buf_B; b.items = h->d_buf_items; b.leaf = h->d_buf_leaf; b.n_leaf = h->d_buf_nleaf; b.l = h->d_buf_l; b.scratch = h->d_buf_scratch;
+    return b;
+}
+
+int pct_set_buffer(pct_handle h, int32_t B) {
+    if (!h) return PCT_ERR_INVALID;
+    if (h->did_reset) { h->err = "pct_set_buffer after a reset: call it between pct_create and the first reset"; return PCT_ERR_STATE; }
+    if (B < 1 || B > BUF_MAX) { h->err = "pct_set_buffer: B must be in [1, 16]"; return PCT_ERR_INVALID; }
+    if (h->cfg.no_auto_reset) { h->err = "pct_set_buffer: buffered envs auto-reset (no_auto_reset = 1 is not supported)"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    cudaFree(h->d_buf_items); cudaFree(h->d_buf_leaf); cudaFree(h->d_buf_nleaf); cudaFree(h->d_buf_l); cudaFree(h->d_buf_scratch);
+    h->d_buf_items = nullptr; h->d_buf_leaf = nullptr; h->d_buf_nleaf = nullptr; h->d_buf_l = nullptr; h->d_buf_scratch = nullptr;
+    h->buf_B = 0;
+    const bool disc = h->cfg.domain == PCT_DISCRETE;
+    const size_t n = (size_t)h->n_envs, slots = n * (size_t)B;
+    CK(h, cudaMalloc(&h->d_buf_items, sizeof(double) * 4 * slots));
+    CK(h, cudaMalloc(&h->d_buf_leaf, (disc ? sizeof(int16_t) : sizeof(double)) * NL_MAX * 6 * slots));
+    CK(h, cudaMalloc(&h->d_buf_nleaf, sizeof(int32_t) * slots));
+    CK(h, cudaMemset(h->d_buf_nleaf, 0, sizeof(int32_t) * slots));
+    CK(h, cudaMalloc(&h->d_buf_l, sizeof(int32_t) * n));
+    CK(h, cudaMalloc(&h->d_buf_scratch, (disc ? sizeof(BufSlotD) : sizeof(BufSlotC)) * slots));
+    h->buf_B = B;
+    return PCT_OK;
+}
+
+int32_t pct_buffer_obs_len(pct_handle h) {
+    if (!h || !h->buf_B) return 0;
+    return (h->cfg.internal_node_holder + h->buf_B * h->cfg.leaf_node_holder + h->buf_B) * 9;
+}
+
+static int check_buffered(pct_handle h, const char *what, bool after_reset) {
+    if (!h->buf_B) { h->err = std::string(what) + ": not a buffered handle (call pct_set_buffer after pct_create)"; return PCT_ERR_STATE; }
+    if (after_reset && !h->did_reset) { h->err = std::string(what) + " before pct_buffer_reset"; return PCT_ERR_STATE; }
+    return PCT_OK;
+}
+
+// select (step only), the apply kernel (reset mode without flat indices), refill + expansion, on stream st
+static int launch_buffered(pct_handle h, const int32_t *flat, void *obs, float *rew, uint8_t *done, pct_step_info *info, cudaStream_t st) {
+    BufParams b = buffer_params(h);
+    b.flat = flat; b.done = flat ? done : nullptr; b.obs = obs; b.info = info;
+    const int mode = flat ? 1 : 0;
+    if (h->cfg.domain == PCT_CONTINUOUS) {
+        CParams p = continuous_params(h);
+        p.leaf_idx = h->d_buf_l; p.reward = rew; p.done = done; p.info = info; p.mode = mode; p.aux = h->d_aux;
+        if (flat) CK(h, launch_buffer_select_continuous(p, b, st));
+        CK(h, launch_apply_continuous(p, h->alias_mode ? PCT_OPT_ALIAS : 0, st));
+        CK(h, launch_buffer_expand_continuous(p, b, st));
+    } else {
+        DParams p = discrete_params(h, 0, h->n_envs);
+        p.leaf_idx = h->d_buf_l; p.reward = rew; p.done = done; p.info = info; p.mode = mode;
+        if (h->d_aux) { p.aux = h->d_aux; p.opt = h->alias_mode ? PCT_OPT_ALIAS : 0; }
+        if (flat) CK(h, launch_buffer_select_discrete(p, b, st));
+        CK(h, launch_apply_discrete(p, st));
+        CK(h, launch_buffer_expand_discrete(p, b, st));
+    }
+    h->launches += flat ? 4 : 3;
+    return PCT_OK;
+}
+
+int pct_buffer_reset(pct_handle h, void *d_obs, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_reset", false);
+    if (rc) return rc;
+    if (!d_obs) { h->err = "pct_buffer_reset: d_obs is NULL"; return PCT_ERR_INVALID; }
+    rc = check_item_source(h);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    rc = launch_buffered(h, nullptr, d_obs, nullptr, nullptr, d_info, (cudaStream_t)stream);
+    if (rc == PCT_OK) h->did_reset = true;
+    return rc;
+}
+
+int pct_buffer_step(pct_handle h, const int32_t *d_leaf_idx, void *d_obs, float *d_reward, uint8_t *d_done, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_step", true);
+    if (rc) return rc;
+    if (!d_leaf_idx || !d_obs || !d_reward || !d_done) { h->err = "pct_buffer_step: d_leaf_idx, d_obs, d_reward and d_done must not be NULL"; return PCT_ERR_INVALID; }
+    rc = check_item_source(h);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    return launch_buffered(h, d_leaf_idx, d_obs, d_reward, d_done, d_info, (cudaStream_t)stream);
+}
+
+int pct_buffer_items(pct_handle h, const int32_t *d_env, int32_t n, double *d_out, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_items", true);
+    if (rc) return rc;
+    if (n < 0) { h->err = "pct_buffer_items: n must be >= 0"; return PCT_ERR_INVALID; }
+    if (n == 0) return PCT_OK;
+    if (!d_out) { h->err = "pct_buffer_items: d_out is NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    CK(h, launch_buffer_items(buffer_params(h), h->n_envs, d_env, n, d_out, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
+int pct_buffer_policy_random(pct_handle h, int32_t *d_idx, uint64_t seed, const int64_t *d_t, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_policy_random", true);
+    if (rc) return rc;
+    if (!d_idx || !d_t) { h->err = "pct_buffer_policy_random: d_idx and d_t must not be NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    CK(h, launch_buffer_policy_random(buffer_params(h), h->n_envs, h->cfg.leaf_node_holder, h->cfg.env_id_base, seed, d_t, d_idx, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
 int64_t pct_snapshot_bytes(pct_handle h) { return h ? snapshot_record_bytes(h) : 0; }
 
 int pct_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_snapshot")) return PCT_ERR_STATE;
     if (!d_buf || n < 0 || ((uintptr_t)d_buf & 15)) { h->err = "pct_snapshot: d_buf must be a 16-byte aligned device buffer and n >= 0"; return PCT_ERR_INVALID; }
     if (!h->did_reset) { h->err = "pct_snapshot before pct_reset"; return PCT_ERR_STATE; }
     if (n == 0) return PCT_OK;
@@ -890,6 +1021,7 @@ int pct_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, voi
 
 int pct_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_t n, const void *d_buf, void *d_obs, void *stream) {
     if (!h) return PCT_ERR_INVALID;
+    if (refuse_buffered(h, "pct_restore")) return PCT_ERR_STATE;
     if (!d_buf || n < 0 || ((uintptr_t)d_buf & 15)) { h->err = "pct_restore: d_buf must be a 16-byte aligned device buffer and n >= 0"; return PCT_ERR_INVALID; }
     if (!h->did_reset) { h->err = "pct_restore before pct_reset"; return PCT_ERR_STATE; }
     if (n == 0) return PCT_OK;

@@ -1,0 +1,432 @@
+// Buffered packing (pct_set_buffer / pct_buffer_*, include/pct_b200.h; DESIGN.md section 18): every env holds B items, and one step picks
+// the item and its placement by a flat index j * NL + l into the leaf blocks of all B items.
+//
+// A step is four launches in plain stream order:
+//   select   warp / env             decode (j, l); buffer item j becomes the env's current item (as pct_set_items writes it, without an
+//                                   expansion) and stored leaf block j the env's leaf list; l goes to the apply kernel's leaf index
+//   apply    the step's own kernel  (pct_discrete.cu / pct_continuous.cu, unchanged) placement, reward, done, info, the draw on success,
+//                                   the auto-reset
+//   refill   thread / env           slot j <- the draw the step consumed; after a reset, slot 0 <- the reset's draw and B - 1 more draws
+//   expand   block / (env, slot)    the leaves of the slot's item on the env's new state with the leaf expansion's routines (stage_env_d,
+//                                   build_candidates and the generators / PCTC_CANDIDATES_BODY, shuffle_candidates, place_virtual_d / _c,
+//                                   first_feasible); the stored leaf block, every observation row of the slot, the record's sums
+// The refill is a kernel of its own because the slots' blocks all read the env's final draw position (the shuffle key).  A reset is the apply
+// kernel's reset mode followed by refill and expand.
+//
+// Scratch of the expansion: the slots of one env run in different blocks, so each slot has its own candidate list and generator / shuffle
+// scratch (BufSlotD / BufSlotC); the rare many-support visits of all of them share the env's BigScratch under the env's lock (DEnvCold::lock,
+// CEnv::lock), as the pooled walks of a step do.  The env record is only read, but for the sums and the sticky flags (atomics).
+#include "pct_common.cuh"
+#include "pct_stability.cuh"
+#include "pct_kernels.h"
+#include "pct_geom.cuh"
+#include "pct_rot.cuh"
+#include "pct_cand.cuh"
+#include "pct_geom_continuous.cuh"
+#include "pct_continuous.cuh"
+#include "pct_cand_c.cuh"
+#include "pct_block.cuh"
+#include "pct_draw.cuh"
+
+// 1: one block per env takes its slots in turn (the layout of pct_expand_kernel); 0: one block per (env, slot).  A/B guard of the measurement
+// in DESIGN.md section 18, not an option of the library.
+#ifndef BUF_SLOTS_INTURN
+#define BUF_SLOTS_INTURN 0
+#endif
+
+namespace pct {
+
+constexpr int BUF_THREADS = 64;
+
+// flat leaf index -> (slot, leaf index of the slot); outside [0, B * nl): slot 0 with the zero action of a plain step
+__device__ __forceinline__ void buf_decode(int d, int B, int nl, int &j, int &l) {
+    if (d < 0 || d >= B * nl) { j = 0; l = -1; }
+    else { j = d / nl; l = d - j * nl; }
+}
+
+// ---- select ----------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) pct_buf_select_kernel(const DParams p, const BufParams b) {
+    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (e >= p.n_envs) return;  // the whole warp
+    int j, l;
+    buf_decode(b.flat[e], b.B, p.nl, j, l);
+    const size_t s = (size_t)e * b.B + j;
+    const int n = b.n_leaf[s];
+    const int16_t *src = (const int16_t *)b.leaf + s * NL_MAX * 6;
+    int16_t *dst = &p.cold[e].leaf[0][0];
+    for (int t = lane; t < n * 6; t += 32) dst[t] = src[t];
+    if (lane == 0) {
+        DHdr &h = p.hot[e].h;
+        const double *it = b.items + s * 4;
+        h.next_box[0] = (int)it[0]; h.next_box[1] = (int)it[1]; h.next_box[2] = (int)it[2];  // what draw_item wrote into the header
+        h.next_den = it[3];
+        h.n_leaf = n;
+        b.l[e] = l;
+    }
+}
+
+__global__ void __launch_bounds__(256) pctc_buf_select_kernel(const CParams p, const BufParams b) {
+    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (e >= p.n_envs) return;
+    int j, l;
+    buf_decode(b.flat[e], b.B, p.nl, j, l);
+    const size_t s = (size_t)e * b.B + j;
+    const int n = b.n_leaf[s];
+    const double *src = (const double *)b.leaf + s * NL_MAX * 6;
+    CEnv *ev = p.env + e;
+    double *dst = &ev->leaf[0][0];
+    for (int t = lane; t < n * 6; t += 32) dst[t] = src[t];
+    if (lane == 0) {
+        const double *it = b.items + s * 4;
+        ev->h.next_box[0] = it[0]; ev->h.next_box[1] = it[1]; ev->h.next_box[2] = it[2];
+        ev->h.next_den = it[3];
+        ev->h.n_leaf = n;
+        b.l[e] = l;
+    }
+}
+
+// ---- refill ----------------------------------------------------------------------------------------------------------------------
+// slot j <- the header's item (the draw the step consumed, or the reset's draw in slot 0 and B - 1 more draws); the header keeps the item it
+// had before the extra draws.  Zeroes the header's leaf / candidate counts, which the expansion sums over the slots.
+template <typename P, typename Hdr, typename Draw>
+__device__ __forceinline__ void buf_refill(const P &p, const BufParams &b, int e, Hdr &h, Draw draw) {
+    double *it = b.items + (size_t)e * b.B * 4;
+    auto put = [&](int j) {
+        it[j * 4 + 0] = (double)h.next_box[0]; it[j * 4 + 1] = (double)h.next_box[1]; it[j * 4 + 2] = (double)h.next_box[2];
+        it[j * 4 + 3] = h.next_den;
+    };
+    if (!b.done || b.done[e]) {
+        put(0);
+        const Hdr h0 = h;
+        for (int j = 1; j < b.B; j++) {
+            draw(h);
+            put(j);
+        }
+        const int64_t dp = h.draw_pos;
+        h = h0;
+        h.draw_pos = dp;
+    } else {
+        int j, l;
+        buf_decode(b.flat[e], b.B, p.nl, j, l);
+        put(j);
+    }
+    h.n_leaf = 0;
+    h.n_cand = 0;
+}
+
+__global__ void __launch_bounds__(128) pct_buf_refill_kernel(const DParams p, const BufParams b) {
+    const int e = blockIdx.x * 128 + threadIdx.x;
+    if (e >= p.n_envs) return;
+    DHdr h = p.hot[e].h;
+    buf_refill(p, b, e, h, [&](DHdr &hh) { draw_item(p, e, hh); });
+    p.hot[e].h = h;
+}
+
+__global__ void __launch_bounds__(128) pctc_buf_refill_kernel(const CParams p, const BufParams b) {
+    const int e = blockIdx.x * 128 + threadIdx.x;
+    if (e >= p.n_envs) return;
+    CHdr h = p.env[e].h;
+    buf_refill(p, b, e, h, [&](CHdr &hh) { draw_item_c(p, e, hh); });
+    p.env[e].h = h;
+}
+
+// ---- expand ----------------------------------------------------------------------------------------------------------------------
+// the slots of block blockIdx.x: (env, first slot, end)
+__device__ __forceinline__ void buf_slots(int B, int &e, int &j0, int &j1) {
+    if (BUF_SLOTS_INTURN) { e = blockIdx.x; j0 = 0; j1 = B; }
+    else { e = blockIdx.x / B; j0 = blockIdx.x - e * B; j1 = j0 + 1; }
+}
+
+// leaf block j of the observation and the stored block, the item row of slot j, and the slot's share of the record and header sums
+template <typename OT, typename LT, typename Hdr>
+__device__ __forceinline__ void buf_emit_slot(const BufParams &b, int nb, int nl, double H, int e, int j, OT *obs, const LT (*leaf)[6], int n_leaf,
+                                              int n_cand, int fl, int flags_now, int n_ems, const double sz[3], double den, Hdr *gh, int tid) {
+    const int B = b.B;
+    OT *o = obs + (size_t)(nb + j * nl) * 9;
+#pragma unroll 1
+    for (int f = tid; f < nl * 9; f += BUF_THREADS) {  // the leaf rows of cur_observation (write_obs / write_obs_c)
+        const int k = f / 9, col = f - k * 9;
+        OT v = 0;
+        if (k < n_leaf) {
+            if (col < 5) v = (OT)leaf[k][col];
+            else if (col == 5) v = (OT)H;
+            else if (col == 8) v = 1;
+        }
+        o[f] = v;
+    }
+    LT *dst = (LT *)b.leaf + ((size_t)e * B + j) * NL_MAX * 6;
+    for (int t = tid; t < n_leaf * 6; t += BUF_THREADS) dst[t] = (&leaf[0][0])[t];
+    if (tid < 9) {  // the item row pct_set_items writes (sizes in ascending order)
+        double s0 = sz[0], s1 = sz[1], s2 = sz[2];
+        if (s1 < s0) { double t = s0; s0 = s1; s1 = t; }
+        if (s2 < s1) { double t = s1; s1 = s2; s2 = t; }
+        if (s1 < s0) { double t = s0; s0 = s1; s1 = t; }
+        const int col = tid;
+        OT v = 0;
+        if (col == 0) v = (OT)den;
+        else if (col == 3) v = (OT)s0;
+        else if (col == 4) v = (OT)s1;
+        else if (col == 5) v = (OT)s2;
+        else if (col == 8) v = 1;
+        obs[(size_t)(nb + B * nl + j) * 9 + col] = v;
+    }
+    if (tid == 0) {
+        b.n_leaf[(size_t)e * B + j] = n_leaf;
+        atomicAdd(&gh->n_leaf, n_leaf);
+        atomicAdd(&gh->n_cand, n_cand);
+        if (fl) atomicOr(&gh->flags, fl);
+        if (b.info) {
+            pct_step_info *r = b.info + e;
+            atomicAdd(&r->n_leaf, n_leaf);
+            atomicAdd(&r->n_cand, n_cand);
+            atomicOr(&r->flags, flags_now | fl);
+            if (j == 0) r->n_ems = n_ems;
+        }
+    }
+}
+
+template <typename SlotT>
+struct BufSmD {
+    StageD s;
+    SlotT tabA[TAB_A], tabB[TAB_B];
+    SetStage stg;
+    int16_t leaf[NL_MAX][6];
+    RotTab rt;
+    int fl, n_cand;
+    uint32_t wb[BUF_THREADS / 32];
+};
+
+template <typename OT, bool STAB, typename SlotT>
+__global__ void __launch_bounds__(BUF_THREADS) pct_buf_expand_kernel(const DParams p, const BufParams b) {
+    constexpr int KB = sizeof(SlotT) == 2 ? 4 : 8;
+    __shared__ __align__(16) BufSmD<SlotT> s;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, B = b.B, nl = p.nl, nb = p.nb;
+    int e, j0, j1;
+    buf_slots(B, e, j0, j1);
+    DEnvCold *cold = p.cold + e;
+    StagedD sd = stage_env_d<STAB>(s.s, p, e, false);
+    const DEnvHot *hot = &s.s.hot;
+    const DHdr &h = hot->h;
+    const int n_box = h.n_box, R = p.setting == 2 ? 6 : 2;
+    const RotTab *rt = &s.rt;
+    OT *obs = (OT *)b.obs + (size_t)e * (size_t)((nb + B * nl + B) * 9);
+    if (j0 == 0) {
+#pragma unroll 1
+        for (int f = tid; f < nb * 9; f += BUF_THREADS) {  // the internal-node rows of write_obs
+            const int row = f / 9, col = f - row * 9;
+            OT v = 0;
+            if (row < n_box) {
+                if (col < 6) v = (OT)hot->box[row][col];
+                else if (col == 6) v = p.setting == 3 ? (OT)cold->density[row] : (OT)1;
+                else if (col == 8) v = 1;
+            } else if (row == 0 && col == 8) v = 1;
+            obs[f] = v;
+        }
+    }
+#pragma unroll 1
+    for (int j = j0; j < j1; j++) {
+        BufSlotD *sc = (BufSlotD *)b.scratch + (size_t)e * B + j;
+        SlotT *const out = (SlotT *)sc->cand;
+        const double *itd = b.items + ((size_t)e * B + j) * 4;
+        const int nb3[3] = {(int)itd[0], (int)itd[1], (int)itd[2]};
+        const double den = itd[3];
+        if (warp == 0) {
+            // ---- the candidates kernel's list for this item, as pct_expand_kernel builds it ----
+            if (lane == 0) make_rot_tab(nb3, R, s.rt);
+            __syncwarp();
+            SlotT *cand = nullptr;
+            int fl = 0, n_cand = 0;
+            if (p.lnes == 0) {
+                const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, lane);
+                cand = cl.keys; n_cand = cl.n; fl = cl.flags;
+            } else {
+                uint32_t *raw = sc->raw;
+                RawList rl;
+                if (p.lnes == 4) rl = gen_full_coord<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, raw, lane);
+                else if (p.lnes == 1) rl = RawList{gen_event_point<KB>(rt, R, p.W, p.L, raw, lane), 0};
+                else rl = gen_level_points<KB>(hot->box, n_box, rt, R, p.W, p.L, p.H, p.lnes == 2, raw, lane);
+                fl = rl.flags;
+                if (rl.n == -2) {  // empty bin under EP / CP: the reference's 2-element list (D:space.py:700-701)
+                    if (lane < 2) out[lane] = (SlotT)key_pack<KB>(0, 0, 0, rt->canon[lane]);
+                    n_cand = 2;
+                    cand = out;
+                } else {
+                    const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, lane, raw, rl.n);
+                    cand = cl.keys; n_cand = cl.n; fl |= cl.flags;
+                }
+            }
+            if (cand != out)
+                for (int t = lane; t < n_cand; t += 32) out[t] = cand[t];
+            __syncwarp();
+            if (p.shuffle)  // the step's keys (seed, global env id, draw_pos) on the slot's scratch (raw + tab_big, as the candidates kernel)
+                shuffle_candidates<SlotT>(out, n_cand, (uint64_t *)sc->raw, (SlotT *)((char *)sc->raw + 10240), p.seed, (uint64_t)(p.env_id_base + e),
+                                          (uint64_t)h.draw_pos, lane);
+            if (lane == 0) { s.n_cand = n_cand; s.fl = fl; }
+        }
+        __syncthreads();
+        // ---- get_possible_position: first `nl` feasible candidates in order ----
+        const int n_cand = s.n_cand;
+        int fl = 0;
+        const int n_leaf = first_feasible<BUF_THREADS / 32>(n_cand, nl, s.leaf, s.wb, [&](int c, int16_t *row) {
+            int xs, ys, zs, rot, mh;
+            key_unpack<KB>(out[c], xs, ys, zs, rot);
+            const int sx = rt->d[rot][0], sy = rt->d[rot][1], sz = rt->d[rot][2];
+            const bool feas = place_virtual_d<STAB>(p, sd.g, sd.pool, &cold->big, &cold->lock, sx, sy, sz, xs, ys, den, mh, fl) != 0;
+            row[0] = (int16_t)xs; row[1] = (int16_t)ys; row[2] = (int16_t)zs;
+            row[3] = (int16_t)(xs + sx); row[4] = (int16_t)(ys + sy); row[5] = (int16_t)(zs + sz);
+            return feas;
+        });
+        fl = __reduce_or_sync(FULL, fl);
+        if (fl && lane == 0) atomicOr(&s.fl, fl);
+        __syncthreads();
+        const double sz[3] = {(double)nb3[0], (double)nb3[1], (double)nb3[2]};
+        buf_emit_slot<OT, int16_t>(b, nb, nl, (double)p.H, e, j, obs, s.leaf, n_leaf, n_cand, s.fl, h.flags, h.n_ems, sz, den, &p.hot[e].h, tid);
+        __syncthreads();  // the next slot reuses the rotation table, the leaves and the flags
+    }
+}
+
+template <typename OT, bool STAB>
+__global__ void __launch_bounds__(BUF_THREADS) pctc_buf_expand_kernel(const CParams p, const BufParams b) {
+    __shared__ uint32_t tabA[CC_TAB], tabB[512];
+    __shared__ uint64_t stg_h[32], rs_h[32];
+    __shared__ uint32_t rs_c[32];
+    __shared__ uint16_t stg_c[32];
+    __shared__ double leaf[NL_MAX][6];
+    __shared__ uint32_t wb[BUF_THREADS / 32];
+    __shared__ int s_fl, s_cnt;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, B = b.B, nl = p.nl, NB = p.nb;
+    int e, j0, j1;
+    buf_slots(B, e, j0, j1);
+    CEnv *env = p.env + e;
+    const CHdr &h = env->h;
+    const int R = p.setting == 2 ? 6 : 2, n_ems = h.n_ems, n_box = h.n_box, flags_now = h.flags;
+    GeomC g{env->box, env->den, n_box};
+    EdgePool pool{env->e_lower, env->e_next, env->e_off, env->first_in, env->last_in, env->e_st, env->e_st, h.n_edge,
+                  env->poly_off, &env->poly[0][0], &env->poly[0][0], h.n_poly};
+    OT *obs = (OT *)b.obs + (size_t)e * (size_t)((NB + B * nl + B) * 9);
+    if (j0 == 0) {
+#pragma unroll 1
+        for (int f = tid; f < NB * 9; f += BUF_THREADS) {  // the internal-node rows of write_obs_c
+            const int row = f / 9, col = f - row * 9;
+            double v = 0;
+            if (row < n_box) {
+                const double *bx = env->box[row];
+                if (col < 3) v = bx[col];
+                else if (col < 6) v = bx[col - 3] + bx[col];
+                else if (col == 8) v = 1;
+            } else if (row == 0 && col == 8) v = 1;
+            obs[f] = (OT)v;
+        }
+    }
+#pragma unroll 1
+    for (int j = j0; j < j1; j++) {
+        BufSlotC *sc = (BufSlotC *)b.scratch + (size_t)e * B + j;
+        // PCTC_CANDIDATES_BODY reads the env's EMS list through `ev` and writes the list and the shuffle scratch through it: here the slot's own
+        struct SlotView {
+            const double (&ems)[CE_MAX][6];
+            uint16_t (&cand)[1232];
+            double (&ems_tmp)[265][6];
+        } view{env->ems, sc->cand, sc->shuf};
+        const SlotView *ev = &view;
+        const double *itd = b.items + ((size_t)e * B + j) * 4;
+        const double nb[3] = {itd[0], itd[1], itd[2]};
+        const double den = itd[3];
+        if (warp == 0) {
+            int fl = 0;
+            PCTC_CANDIDATES_BODY
+            if (lane == 0) { s_cnt = cnt; s_fl = fl; }
+        }
+        __syncthreads();
+        const int n_cand = s_cnt;
+        int fl = 0;
+        const int n_leaf = first_feasible<BUF_THREADS / 32>(n_cand, nl, leaf, wb, [&](int c, double *t6) {
+            cand_tuple(sc->cand[c], env->ems, nb, t6);
+            double mh;
+            return place_virtual_c<STAB>(p, g, pool, &env->big, &env->lock, t6[3] - t6[0], t6[4] - t6[1], t6[5] - t6[2], t6[0], t6[1], den, mh, fl) != 0;
+        });
+        fl = __reduce_or_sync(FULL, fl);
+        if (fl && lane == 0) atomicOr(&s_fl, fl);
+        __syncthreads();
+        buf_emit_slot<OT, double>(b, NB, nl, p.H, e, j, obs, leaf, n_leaf, n_cand, s_fl, flags_now, n_ems, nb, den, &env->h, tid);
+        __syncthreads();
+    }
+}
+
+// ---- policy and items ------------------------------------------------------------------------------------------------------------
+__global__ void pct_buf_policy_random_kernel(const BufParams b, int n_envs, int nl, int64_t env_id_base, uint64_t seed, const int64_t *t_dev,
+                                             int32_t *idx) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_envs) return;
+    const int32_t *nlf = b.n_leaf + (size_t)e * b.B;
+    int total = 0;
+    for (int j = 0; j < b.B; j++) total += nlf[j];
+    if (total == 0) { idx[e] = 0; return; }
+    int k = (int)(rnd_u64(seed, (uint64_t)(env_id_base + e), (uint64_t)*t_dev) % (uint64_t)total), j = 0;
+    while (k >= nlf[j]) { k -= nlf[j]; j++; }
+    idx[e] = j * nl + k;
+}
+
+__global__ void pct_buf_items_kernel(const BufParams b, int n_envs, const int32_t *env, int n, double *out) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (int64_t)n * b.B * 4) return;
+    const int r = (int)(t / (b.B * 4)), q = (int)(t - (int64_t)r * b.B * 4);
+    const int e = env ? env[r] : r;
+    out[t] = (e >= 0 && e < n_envs) ? b.items[(size_t)e * b.B * 4 + q] : 0.0;
+}
+
+// ---- launchers -------------------------------------------------------------------------------------------------------------------
+static unsigned buf_blocks(int n_envs, int B) { return BUF_SLOTS_INTURN ? (unsigned)n_envs : (unsigned)n_envs * (unsigned)B; }
+
+cudaError_t launch_buffer_select_discrete(const DParams &p, const BufParams &b, cudaStream_t st) {
+    pct_buf_select_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b, cudaStream_t st) {
+    pctc_buf_select_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b);
+    return cudaGetLastError();
+}
+
+template <typename OT, bool STAB>
+static void expand_d(const DParams &p, const BufParams &b, cudaStream_t st) {
+    const bool small = p.W <= 16 && p.L <= 16 && p.H <= 16;  // the candidate key width of the step (launch_s)
+    const unsigned g = buf_blocks(p.n_envs, b.B);
+    if (small) pct_buf_expand_kernel<OT, STAB, uint16_t><<<g, BUF_THREADS, 0, st>>>(p, b);
+    else pct_buf_expand_kernel<OT, STAB, uint32_t><<<g, BUF_THREADS, 0, st>>>(p, b);
+}
+
+cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st) {
+    pct_buf_refill_kernel<<<(p.n_envs + 127) / 128, 128, 0, st>>>(p, b);
+    const bool stab = p.setting != 2;
+    if (p.obs_f64) { if (stab) expand_d<double, true>(p, b, st); else expand_d<double, false>(p, b, st); }
+    else { if (stab) expand_d<float, true>(p, b, st); else expand_d<float, false>(p, b, st); }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st) {
+    pctc_buf_refill_kernel<<<(p.n_envs + 127) / 128, 128, 0, st>>>(p, b);
+    const bool stab = p.setting != 2;
+    const unsigned g = buf_blocks(p.n_envs, b.B);
+    if (p.obs_f64) {
+        if (stab) pctc_buf_expand_kernel<double, true><<<g, BUF_THREADS, 0, st>>>(p, b);
+        else pctc_buf_expand_kernel<double, false><<<g, BUF_THREADS, 0, st>>>(p, b);
+    } else {
+        if (stab) pctc_buf_expand_kernel<float, true><<<g, BUF_THREADS, 0, st>>>(p, b);
+        else pctc_buf_expand_kernel<float, false><<<g, BUF_THREADS, 0, st>>>(p, b);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_items(const BufParams &b, int n_envs, const int32_t *env, int n, double *out, cudaStream_t st) {
+    const int64_t total = (int64_t)n * b.B * 4;
+    pct_buf_items_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(b, n_envs, env, n, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_policy_random(const BufParams &b, int n_envs, int nl, int64_t env_id_base, uint64_t seed, const int64_t *t_dev,
+                                        int32_t *idx, cudaStream_t st) {
+    pct_buf_policy_random_kernel<<<(n_envs + 127) / 128, 128, 0, st>>>(b, n_envs, nl, env_id_base, seed, t_dev, idx);
+    return cudaGetLastError();
+}
+
+}  // namespace pct

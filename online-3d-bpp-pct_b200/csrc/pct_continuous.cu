@@ -18,33 +18,12 @@
 #include "pct_continuous.cuh"
 #include "pct_cand_c.cuh"
 #include "pct_block.cuh"
+#include "pct_draw.cuh"
 
 namespace pct {
 
 // around6, NodeC / GeomC (geometry policy of the stability routine), rest_height_c, rest_height_pre: pct_geom_continuous.cuh
 // rot_dims_c, cand_tuple, hash_double_call, cand_hash_c, cand_equal and the set emulation (PCTC_CANDIDATES_BODY): pct_cand_c.cuh
-
-__device__ __noinline__ void draw_item_c(const CParams &p, int e, CHdr &h) {
-    const uint64_t gid = (uint64_t)(p.env_id_base + e), d = (uint64_t)h.draw_pos;
-    if (p.item_mode == 0 && p.sample_dist) {  // C:bin3D.py:103-112
-        auto u01 = [&](uint64_t salt) { return (double)(rnd_u64(p.seed ^ salt, gid, d) >> 11) * (1.0 / 9007199254740992.0); };
-        auto r3 = [&](double v) { return ddiv(rint(v * 1000.0), 1000.0); };
-        h.next_box[0] = r3(p.sample_a + (p.sample_b - p.sample_a) * u01(0x11));
-        h.next_box[1] = r3(p.sample_a + (p.sample_b - p.sample_a) * u01(0x22));
-        if (p.setting == 2) h.next_box[2] = r3(p.sample_a + (p.sample_b - p.sample_a) * u01(0x33));
-        else {
-            const double ch[5] = {0.1, 0.2, 0.3, 0.4, 0.5};
-            h.next_box[2] = ch[rnd_u64(p.seed ^ 0x44, gid, d) % 5];
-        }
-        h.next_den = p.setting == 3 ? rnd_density(p.seed, gid, d) : 1.0;
-    } else {
-        const double *it = p.item_mode == 0 ? p.item_set + (rnd_u64(p.seed, gid, d) % (uint64_t)p.n_items) * 3
-                                            : p.stream + ((size_t)e * p.stream_len + (size_t)(d % (uint64_t)p.stream_len)) * 4;
-        h.next_box[0] = it[0]; h.next_box[1] = it[1]; h.next_box[2] = it[2];
-        h.next_den = p.setting == 3 ? (p.item_mode == 0 ? rnd_density(p.seed, gid, d) : it[3]) : 1.0;
-    }
-    h.draw_pos++;
-}
 
 __device__ __noinline__ void reset_space_c(CEnv *ev, const CParams &p, int e, int lane) {
     if (lane == 0) {
@@ -801,6 +780,15 @@ cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetP
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;
     return launch_continuous(p, opt, st, false, sel);
+}
+
+// the apply kernel alone, in plain stream order (pct_buffer_step / pct_buffer_reset)
+cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st) {
+    const int b2 = (p.n_envs + 1) / 2;
+    if (p.setting != 2 && (opt & PCT_OPT_ALIAS)) pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);
+    else if (p.setting != 2) pctc_apply_kernel<true, false><<<b2, 64, 0, st>>>(p);
+    else pctc_apply_kernel<false, false><<<b2, 64, 0, st>>>(p);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st) {

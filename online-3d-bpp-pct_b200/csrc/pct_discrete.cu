@@ -1038,6 +1038,24 @@ cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof
     return stab ? launch_s<float, true>(p, st, prof, apply, sel) : launch_s<float, false>(p, st, prof, apply, sel);
 }
 
+// the apply kernel alone, in plain stream order (pct_buffer_step / pct_buffer_reset: the buffered pipeline's own kernels run around it)
+template <bool STAB>
+static cudaError_t launch_apply_s(const DParams &p, cudaStream_t st) {
+    static bool attr_set = false;
+    const size_t smem1 = (size_t)K1_SM_PER_WARP * WARPS_PER_BLOCK;
+    if (!attr_set) {
+        cudaError_t err = set_smem(pct_apply_kernel<STAB, false>, smem1);
+        if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB>, smem1);
+        if (err != cudaSuccess) return err;
+        attr_set = true;
+    }
+    const int blocks = (p.n_envs + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+    if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+    else pct_apply_kernel<STAB, false><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+    return cudaGetLastError();
+}
+cudaError_t launch_apply_discrete(const DParams &p, cudaStream_t st) { return p.setting != 2 ? launch_apply_s<true>(p, st) : launch_apply_s<false>(p, st); }
+
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                           cudaStream_t st, const int64_t *t_dev) {
     pct_policy_random_kernel<<<(n_envs + 127) / 128, 128, 0, st>>>(hot, n_envs, env_id_base, seed, t, t_dev, leaf_idx);

@@ -60,6 +60,13 @@ struct pct_env_batch {
     pct::QueryOne<double> *d_query_c = nullptr;  // pct_query_placement_f64
     pct::QueryOne<int32_t> *d_query = nullptr;   // pct_query_placement, then HEUR_SIDE_MAX^2 ints for the height map
     int item_mode = 0;
+    // buffered packing (pct_set_buffer; pct_buffer.cu): buf_B > 0 makes the handle a buffered one
+    int buf_B = 0;
+    double *d_buf_items = nullptr;   // [n_envs][B][4]
+    void *d_buf_leaf = nullptr;      // [n_envs][B][NL_MAX][6] int16 / double
+    int32_t *d_buf_nleaf = nullptr;  // [n_envs][B]
+    int32_t *d_buf_l = nullptr;      // [n_envs]
+    void *d_buf_scratch = nullptr;   // [n_envs][B] BufSlotD / BufSlotC
     // staging for the host-buffer entry points
     void *d_obs = nullptr, *d_act = nullptr;
     int32_t *d_idx = nullptr;

@@ -378,4 +378,43 @@ cudaError_t launch_heuristic_continuous(const CParams &p, const HParamsC &hp, cu
 cudaError_t launch_policy_random_continuous(const CEnv *env, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                             cudaStream_t st);
 
+// ---- buffered packing (pct_buffer.cu; DESIGN.md section 18) ----
+constexpr int BUF_MAX = 16;  // buffered items per env
+// per-slot scratch of the buffered expansion, which runs the slots of one env in different blocks: the candidate list and the generator
+// output / shuffle scratch of the step's candidates kernel (DEnvCold::cand / raw / tab_big: raw and tab_big contiguous, as shuffle_candidates uses them)
+struct BufSlotD {
+    uint32_t cand[CAND_MAX];
+    uint32_t raw[2048];
+    uint32_t tab_big[TAB_A];
+};
+// ... of the continuous domain (CEnv::cand, and the 12.4 KB of CEnv::ems_tmp the keyed shuffle uses)
+struct BufSlotC {
+    uint16_t cand[1232];
+    double shuf[265][6];
+};
+struct BufParams {
+    int B;
+    double *items;           // [n_envs][B][4] x, y, z, density of each slot, as drawn
+    void *leaf;              // [n_envs][B][NL_MAX][6] each slot's leaf block, in the format of DEnvCold::leaf (int16) / CEnv::leaf (double)
+    int32_t *n_leaf;         // [n_envs][B]
+    int32_t *l;              // [n_envs] leaf index of the chosen slot: the apply kernel's leaf_idx
+    void *scratch;           // [n_envs][B] BufSlotD / BufSlotC
+    const int32_t *flat;     // step: the caller's flat leaf indices
+    const uint8_t *done;     // step: the apply kernel's done bytes; nullptr (reset): every env was reset
+    void *obs;               // (NB + B * NL + B) * 9 values per env, the observation dtype
+    pct_step_info *info;     // or nullptr
+};
+// the apply kernel alone (whole batch, plain stream order, p.order = p.ready = nullptr): pct_buffer_step / pct_buffer_reset
+cudaError_t launch_apply_discrete(const DParams &p, cudaStream_t st);
+cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st);
+// the select kernel (chosen slot's item and leaf block -> the env), before the apply kernel
+cudaError_t launch_buffer_select_discrete(const DParams &p, const BufParams &b, cudaStream_t st);
+cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b, cudaStream_t st);
+// refill and expansion of every slot, the observation and the records, after the apply kernel
+cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st);
+cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st);
+cudaError_t launch_buffer_items(const BufParams &b, int n_envs, const int32_t *env, int n, double *out, cudaStream_t st);
+cudaError_t launch_buffer_policy_random(const BufParams &b, int n_envs, int nl, int64_t env_id_base, uint64_t seed, const int64_t *t_dev,
+                                        int32_t *idx, cudaStream_t st);
+
 }  // namespace pct

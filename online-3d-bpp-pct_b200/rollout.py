@@ -28,6 +28,16 @@ def drl_gat_policy(net, tools, internal_node_holder=80, leaf_node_holder=50, nor
     return policy
 
 
+def buffered_drl_gat(net, B, internal_node_holder=80, leaf_node_holder=50):
+    """The reference's DRL_GAT on a buffered batch (PctBatch(..., buffer=B)): `net` is built with leaf_node_holder = B * NL (the leaf
+    blocks of the B items are one leaf list to its pointer), and its encoder's graph_size, fixed at construction, becomes the node count of
+    a buffered observation, NB + B * NL + B (graph_encoder.py: `graph_size`).  The item rows after the leaf blocks are read as next-item rows
+    by observation_decode_leaf_node (tools.py) and embedded by AttentionModel.forward as they are.  Drive it with
+    drl_gat_policy(net, tools, internal_node_holder, B * leaf_node_holder); its leaf index is the batch's flat index j * NL + l."""
+    net.actor.embedder.graph_size = int(internal_node_holder) + int(B) * int(leaf_node_holder) + int(B)
+    return net
+
+
 class GraphedRollout(object):
     """policy: callable(obs (N, obs_len) float32 CUDA tensor, t_dev int64 CUDA scalar tensor) -> int32 CUDA tensor (N,) of leaf indices,
     made of capturable torch ops (e.g. a DRL_GAT forward + argmax / multinomial); None = the built-in uniform-valid-leaf kernel.
