@@ -10,25 +10,7 @@
 namespace pct {
 
 // ---- candidate leaves in CPython set order (EMSPoint, D:space.py:534-570) ---------------------------------
-// set_insert_clean (setobject.c) for a key known to be absent: plain scalar probe loop, run by ONE lane
-template <typename SlotT>
-__device__ __forceinline__ void table_insert_clean(SlotT *tab, uint32_t mask, uint64_t hash, SlotT key) {
-    uint64_t perturb = hash;
-    uint32_t i = (uint32_t)hash & mask;
-#pragma unroll 1
-    for (;;) {
-        if (tab[i] == (SlotT)~(SlotT)0) { tab[i] = key; return; }
-        if (i + 9 <= mask) {
-#pragma unroll 1
-            for (int j = 1; j <= 9; j++)
-                if (tab[i + j] == (SlotT)~(SlotT)0) { tab[i + j] = key; return; }
-        }
-        perturb >>= 5;
-        i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;
-    }
-}
-
-struct SetStage {  // per-warp staging of (hash, key) pairs for the serial insertion
+struct SetStage {  // per-warp staging area of the candidates kernel's shared-memory layout; build_candidates does not use it
     uint64_t h[32];
     uint32_t k[32];
 };
@@ -41,16 +23,17 @@ struct CandList {
     int n, flags;
 };
 
-// Inserting a key that is already in the set is a no-op, so only FIRST occurrences have to go through the
-// order-defining serial insertion: every lane first looks its key up in the current table (read-only, the
-// lookup of a present key follows exactly the probe sequence that placed it), duplicates inside the 32-wide
-// chunk are collapsed onto their lowest lane with __match_any_sync, the surviving new keys are compacted into a
-// shared-memory staging buffer in lane (= reference insertion) order and inserted by lane 0 with a scalar
-// set_insert_clean (the kernel is instruction-issue bound: a one-lane scalar loop costs ~3x fewer warp
-// instructions than a ballot-based warp-wide probe).  Resizes re-hash the old table in parallel, 32 slots at a time.
+// Inserting a key that is already in the set is a no-op, so only FIRST occurrences change the table: duplicates inside the 32-wide chunk
+// are collapsed onto their lowest lane with __match_any_sync, and every lane walks its key's probe sequence in the table as it stood at
+// the chunk's start (a present key is found on exactly the sequence that placed it).  A new key's walk stops on the first empty slot of
+// its sequence, which is where set_add_entry would put it if no lane below had gone first.  The new keys then go in by claim rounds
+// (set_claim_round, pct_common.cuh): each round commits, in one step, the lanes whose serial insertion in lane (= reference) order
+// would land on the slot they stand on, and the others walk on from there.  A resize re-inserts the old table 32 slots at a time by the
+// same rounds (set_rehash), and the keys still pending walk the new table from their home slots.
 template <typename SlotT>
 __device__ __noinline__ CandList<SlotT> build_candidates(const int16_t (*ems)[6], int n_ems, const RotTab *rt, int R, SlotT *tabA, SlotT *tabB, SlotT *tabBig,
                                                          SetStage *stg, int lane, const uint32_t *raw_keys = nullptr, int n_raw = 0) {
+    (void)stg;
     constexpr int BITS = sizeof(SlotT) == 2 ? 4 : 8;
     constexpr SlotT EMPTY = (SlotT)~(SlotT)0;
     SlotT *tab = tabA;
@@ -88,45 +71,18 @@ __device__ __noinline__ CandList<SlotT> build_candidates(const int16_t (*ems)[6]
         // first occurrence inside the chunk
         const uint32_t same = __match_any_sync(FULL, key);
         if (valid && (same & ((1u << lane) - 1))) valid = false;
-        // already in the set?  (set_add_entry probe sequence, read-only)
-        if (valid) {
-            uint64_t perturb = hash;
-            uint32_t i = (uint32_t)hash & mask;
-            bool open = true;
-            while (open) {
-                const int probes = (i + 9 <= mask) ? 9 : 0;
-                for (int j = 0; j <= probes; j++) {
-                    const SlotT e = tab[i + j];
-                    if (e == EMPTY) { open = false; break; }
-                    if (e == (SlotT)key) { open = false; valid = false; break; }
-                }
-                perturb >>= 5;
-                i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;
-            }
-        }
-        const uint32_t vm = __ballot_sync(FULL, valid);
-        int n_new = __popc(vm);
-        if (valid) {
-            const int pos = __popc(vm & ((1u << lane) - 1));
-            stg->h[pos] = hash;
-            stg->k[pos] = key;
-        }
-        __syncwarp();
-        int done = 0;
+        SetProbe pr;
+        pr.home(hash, mask);
+        // the first pass of the seek is the read-only lookup (a present key drops out); later passes walk on from a lost claim or, after a
+        // resize, from the home slot: the chunk's keys differ from each other and from the table's, so those find nothing equal
 #pragma unroll 1
-        while (done < n_new) {
-            // lane 0: insert staged keys until the set has to grow
-            int upto = n_new;
-            if (lane == 0) {
-#pragma unroll 1
-                for (int t = done; t < n_new; t++) {
-                    table_insert_clean<SlotT>(tab, mask, stg->h[t], (SlotT)stg->k[t]);
-                    if ((uint32_t)(++fill) * 5 >= mask * 3) { upto = t + 1; break; }
-                }
-            }
-            upto = __shfl_sync(FULL, upto, 0);
-            fill = __shfl_sync(FULL, fill, 0);
-            done = upto;
+        for (;;) {
+            if (valid && set_seek(tab, mask, pr, [key](SlotT e) { return e == (SlotT)key; })) valid = false;
+            const uint32_t room = (mask * 3 + 4) / 5 - (uint32_t)fill;  // insertions until fill * 5 >= mask * 3
+            const uint32_t cm = set_claim_round(valid, pr.slot(), lane, room);
+            if (!cm) break;
+            if ((cm >> lane) & 1) { tab[pr.slot()] = (SlotT)key; valid = false; }
+            fill += __popc(cm);
             __syncwarp();
             if ((uint32_t)fill * 5 >= mask * 3) {
                 // set_table_resize(used * 4): smallest power of two > 4 * used, re-insert in slot order
@@ -135,36 +91,11 @@ __device__ __noinline__ CandList<SlotT> build_candidates(const int16_t (*ems)[6]
                 if (newsize > TAB_A) { flags |= PCT_FLAG_CAND_OVERFLOW; stop = true; break; }
                 SlotT *nt = newsize == TAB_A ? tabBig : ((tab == tabA) ? tabB : tabA);
                 for (uint32_t t = lane; t < newsize; t += 32) nt[t] = EMPTY;
-                // the staged keys not inserted yet must survive: move them to registers
-                const uint64_t keep_h = (done + lane < n_new) ? stg->h[done + lane] : 0;
-                const uint32_t keep_k = (done + lane < n_new) ? stg->k[done + lane] : 0;
                 __syncwarp();
-#pragma unroll 1
-                for (uint32_t b2 = 0; b2 <= mask; b2 += 32) {
-                    const uint32_t s = b2 + lane;
-                    const SlotT e = s <= mask ? tab[s] : EMPTY;
-                    const uint32_t em = __ballot_sync(FULL, e != EMPTY);
-                    if (e != EMPTY) {
-                        const int pos = __popc(em & ((1u << lane) - 1));
-                        stg->h[pos] = key_hash<BITS>(e, rt);
-                        stg->k[pos] = e;
-                    }
-                    __syncwarp();
-                    if (lane == 0) {
-                        const int m2 = __popc(em);
-#pragma unroll 1
-                        for (int t = 0; t < m2; t++) table_insert_clean<SlotT>(nt, newsize - 1, stg->h[t], (SlotT)stg->k[t]);
-                    }
-                    __syncwarp();
-                }
+                set_rehash(tab, mask, nt, newsize - 1, lane, [rt](SlotT e) { return key_hash<BITS>(e, rt); });
                 tab = nt;
                 mask = newsize - 1;
-                // restore the pending keys at the front of the staging buffer
-                if (done + lane < n_new) { stg->h[lane] = keep_h; stg->k[lane] = keep_k; }
-                // (indices shift: pending key t now sits at t - done)
-                __syncwarp();
-                n_new -= done;  // the pending keys now sit at staged[0 .. n_new)
-                done = 0;
+                pr.home(hash, mask);
             }
         }
     }

@@ -50,8 +50,8 @@ __device__ __forceinline__ bool cand_equal(uint16_t a, uint16_t b, const double 
 // The set emulation of one warp: the candidate codes of the item `nb` (R orientations) over the EMS list of `ev`, in CPython-set order, into
 // ev->cand (`cnt` of them, declared here), then the keyed shuffle when p.shuffle is set (scratch: ev->ems_tmp).  Expanded in place (a macro, not
 // an inlined function, so that pctc_candidates_kernel keeps its code).  Names it uses from the enclosing scope: p, e, lane, ev, h (the header),
-// nb, R, n_ems, fl (capacity flags, ORed), and the warp's shared arrays uint32_t tabA[CC_TAB], tabB[512], uint64_t stg_h[32], rs_h[32],
-// uint32_t rs_c[32], uint16_t stg_c[32].
+// nb, R, n_ems, fl (capacity flags, ORed), and the warp's shared tables uint32_t tabA[CC_TAB], tabB[512].  The callers' staging arrays
+// (uint64_t stg_h[32], rs_h[32], uint32_t rs_c[32], uint16_t stg_c[32]) belong to their shared-memory layouts; the body no longer uses them.
 #define PCTC_CANDIDATES_BODY                                                                                                                                   \
     constexpr uint32_t EMPTY = 0xFFFFFFFFu;                                                                                                                    \
     uint32_t *tab = tabA;                                                                                                                                      \
@@ -59,6 +59,8 @@ __device__ __forceinline__ bool cand_equal(uint16_t a, uint16_t b, const double 
     int fill = 0;                                                                                                                                              \
     if (lane < 8) tab[lane] = EMPTY;                                                                                                                           \
     __syncwarp();                                                                                                                                              \
+    /* the callers' staging arrays keep their places in the shared-memory layouts, unused */                                                                   \
+    asm volatile("" ::"r"(smem_u32(stg_h)), "r"(smem_u32(rs_h)), "r"(smem_u32(rs_c)), "r"(smem_u32(stg_c)));                                                   \
     const int raw = n_ems * R * 4;                                                                                                                             \
     bool stop = false;                                                                                                                                         \
 _Pragma("unroll 1")                                                                                                                                              \
@@ -99,65 +101,21 @@ _Pragma("unroll 1")                                                             
             l6[2] = __shfl_sync(FULL, h2, gb); l6[5] = __shfl_sync(FULL, h2, gb + 1);                                                                          \
             if (valid) hash = tuple_hash6(l6);                                                                                                                 \
         }                                                                                                                                                      \
-        /* already present? (read-only probe; present keys sit on their own probe sequence) */                                                                 \
-        if (valid) {                                                                                                                                           \
-            const uint32_t tag = (uint32_t)(hash >> 48);                                                                                                       \
-            uint64_t perturb = hash;                                                                                                                           \
-            uint32_t i = (uint32_t)hash & mask;                                                                                                                \
-            bool open = true;                                                                                                                                  \
-            while (open) {                                                                                                                                     \
-                const int probes = (i + 9 <= mask) ? 9 : 0;                                                                                                    \
-                for (int j = 0; j <= probes; j++) {                                                                                                            \
-                    const uint32_t s = tab[i + j];                                                                                                             \
-                    if (s == EMPTY) { open = false; break; }                                                                                                   \
-                    if ((s >> 16) == tag && cand_equal((uint16_t)s, code, ev->ems, nb)) { open = false; valid = false; break; }                                \
-                }                                                                                                                                              \
-                perturb >>= 5;                                                                                                                                 \
-                i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;                                                                                          \
-            }                                                                                                                                                  \
-        }                                                                                                                                                      \
-        /* the new keys of this chunk go through the order-defining insertion in lane (= reference) order: staged in shared memory and inserted by */          \
-        /* lane 0 with a scalar set_add_entry (3x fewer warp instructions than a warp-uniform probe with shuffles, as in the discrete kernel); */              \
-        /* an equal tuple staged by an earlier lane of the same chunk is found by the tag + exact comparison like any other present key */                     \
-        const uint32_t vm = __ballot_sync(FULL, valid);                                                                                                        \
-        const int n_new = __popc(vm);                                                                                                                          \
-        if (valid) {                                                                                                                                           \
-            const int pos = __popc(vm & ((1u << lane) - 1));                                                                                                   \
-            stg_h[pos] = hash;                                                                                                                                 \
-            stg_c[pos] = code;                                                                                                                                 \
-        }                                                                                                                                                      \
-        __syncwarp();                                                                                                                                          \
-        int done = 0;                                                                                                                                          \
+        /* the chunk's new keys go in by claim rounds in lane (= reference) order, as in the discrete build_candidates (pct_cand.cuh).  The first pass */      \
+        /* of the seek is the read-only lookup; a lane that lost a claim walks on with the same tag + exact comparison, so a value-equal tuple of a */         \
+        /* lower lane (equal hash: the same sequence) is met where set_add_entry would meet it, and the higher code drops out */                               \
+        SetProbe pr;                                                                                                                                           \
+        pr.home(hash, mask);                                                                                                                                   \
+        const uint32_t tag = (uint32_t)(hash >> 48);                                                                                                           \
 _Pragma("unroll 1")                                                                                                                                              \
-        while (done < n_new && !stop) {                                                                                                                        \
-            int upto = n_new;                                                                                                                                  \
-            if (lane == 0) {                                                                                                                                   \
-_Pragma("unroll 1")                                                                                                                                              \
-                for (int t = done; t < n_new; t++) {                                                                                                           \
-                    const uint64_t hk = stg_h[t];                                                                                                              \
-                    const uint16_t ck = stg_c[t];                                                                                                              \
-                    const uint32_t tagk = (uint32_t)(hk >> 48);                                                                                                \
-                    uint64_t perturb = hk;                                                                                                                     \
-                    uint32_t i = (uint32_t)hk & mask;                                                                                                          \
-                    int state = 0;                                                                                                                             \
-_Pragma("unroll 1")                                                                                                                                              \
-                    while (!state) {                                                                                                                           \
-                        const int probes = (i + 9 <= mask) ? 9 : 0;                                                                                            \
-_Pragma("unroll 1")                                                                                                                                              \
-                        for (int j = 0; j <= probes; j++) {                                                                                                    \
-                            const uint32_t sl = tab[i + j];                                                                                                    \
-                            if (sl == EMPTY) { tab[i + j] = (tagk << 16) | ck; state = 1; break; }                                                             \
-                            if ((sl >> 16) == tagk && cand_equal((uint16_t)sl, ck, ev->ems, nb)) { state = 2; break; }                                         \
-                        }                                                                                                                                      \
-                        perturb >>= 5;                                                                                                                         \
-                        i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;                                                                                  \
-                    }                                                                                                                                          \
-                    if (state == 1 && (uint32_t)(++fill) * 5 >= mask * 3) { upto = t + 1; break; }                                                             \
-                }                                                                                                                                              \
-            }                                                                                                                                                  \
-            upto = __shfl_sync(FULL, upto, 0);                                                                                                                 \
-            fill = __shfl_sync(FULL, fill, 0);                                                                                                                 \
-            done = upto;                                                                                                                                       \
+        for (;;) {                                                                                                                                             \
+            if (valid && set_seek(tab, mask, pr, [&](uint32_t sl) { return (sl >> 16) == tag && cand_equal((uint16_t)sl, code, ev->ems, nb); }))               \
+                valid = false;                                                                                                                                 \
+            const uint32_t room = (mask * 3 + 4) / 5 - (uint32_t)fill;                                                                                         \
+            const uint32_t cm = set_claim_round(valid, pr.slot(), lane, room);                                                                                 \
+            if (!cm) break;                                                                                                                                    \
+            if ((cm >> lane) & 1) { tab[pr.slot()] = (tag << 16) | code; valid = false; }                                                                      \
+            fill += __popc(cm);                                                                                                                                \
             __syncwarp();                                                                                                                                      \
             if ((uint32_t)fill * 5 >= mask * 3) {                                                                                                              \
                 uint32_t newsize = 8;                                                                                                                          \
@@ -166,43 +124,17 @@ _Pragma("unroll 1")                                                             
                 uint32_t *nt = (tab == tabA) ? tabB : tabA;                                                                                                    \
                 for (uint32_t t = lane; t < newsize; t += 32) nt[t] = EMPTY;                                                                                   \
                 __syncwarp();                                                                                                                                  \
-_Pragma("unroll 1")                                                                                                                                              \
-                for (uint32_t b2 = 0; b2 <= mask; b2 += 32) {  /* set_table_resize: re-insert in slot order (set_insert_clean: no comparisons) */              \
-                    const uint32_t sidx = b2 + lane;                                                                                                           \
-                    const uint32_t c2 = sidx <= mask ? tab[sidx] : EMPTY;                                                                                      \
-                    const uint32_t em = __ballot_sync(FULL, c2 != EMPTY);                                                                                      \
-                    if (c2 != EMPTY) {                                                                                                                         \
-                        double u[6];                                                                                                                           \
-                        cand_tuple((uint16_t)c2, ev->ems, nb, u);                                                                                              \
-                        const int pos = __popc(em & ((1u << lane) - 1));                                                                                       \
-                        rs_h[pos] = cand_hash_c(u);                                                                                                            \
-                        rs_c[pos] = c2;                                                                                                                        \
-                    }                                                                                                                                          \
-                    __syncwarp();                                                                                                                              \
-                    if (lane == 0) {                                                                                                                           \
-                        const int m2 = __popc(em);                                                                                                             \
-_Pragma("unroll 1")                                                                                                                                              \
-                        for (int t = 0; t < m2; t++) {                                                                                                         \
-                            uint64_t pt = rs_h[t];                                                                                                             \
-                            uint32_t ii = (uint32_t)pt & (newsize - 1);                                                                                        \
-                            bool placed = false;                                                                                                               \
-_Pragma("unroll 1")                                                                                                                                              \
-                            while (!placed) {                                                                                                                  \
-                                const int pr = (ii + 9 <= newsize - 1) ? 9 : 0;                                                                                \
-                                for (int j = 0; j <= pr; j++)                                                                                                  \
-                                    if (nt[ii + j] == EMPTY) { nt[ii + j] = rs_c[t]; placed = true; break; }                                                   \
-                                pt >>= 5;                                                                                                                      \
-                                ii = (uint32_t)((uint64_t)ii * 5 + 1 + pt) & (newsize - 1);                                                                    \
-                            }                                                                                                                                  \
-                        }                                                                                                                                      \
-                    }                                                                                                                                          \
-                    __syncwarp();                                                                                                                              \
-                }                                                                                                                                              \
+                /* set_table_resize: re-insert in slot order (set_insert_clean: no comparisons); the slots hold the tag only, so the hash is rebuilt */        \
+                set_rehash(tab, mask, nt, newsize - 1, lane, [&](uint32_t c2) {                                                                                \
+                    double u[6];                                                                                                                               \
+                    cand_tuple((uint16_t)c2, ev->ems, nb, u);                                                                                                  \
+                    return cand_hash_c(u);                                                                                                                     \
+                });                                                                                                                                            \
                 tab = nt;                                                                                                                                      \
                 mask = newsize - 1;                                                                                                                            \
+                pr.home(hash, mask);                                                                                                                           \
             }                                                                                                                                                  \
         }                                                                                                                                                      \
-        __syncwarp();                                                                                                                                          \
     }                                                                                                                                                          \
     __syncwarp();                                                                                                                                              \
     int cnt = 0;                                                                                                                                               \

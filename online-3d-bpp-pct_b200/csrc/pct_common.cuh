@@ -54,6 +54,73 @@ __device__ __forceinline__ uint64_t tuple_hash_n(const uint64_t *lane, int n) {
     if (acc == ~0ull) return 1546275796ull;
     return acc;
 }
+
+// ---- CPython 3.12 set insertion, a warp of keys at a time (the candidate lists: pct_cand.cuh, pct_cand_c.cuh) ----------------------
+// A lane's place on its key's probe sequence (setobject.c, no deletions): home slot hash & mask; from each window start i the slots
+// i .. i + 9 when i + 9 <= mask, else i alone; then perturb >>= 5, i = (i * 5 + 1 + perturb) & mask.
+struct SetProbe {
+    uint64_t perturb;
+    uint32_t i, j;  // window start, offset in the window
+    __device__ __forceinline__ void home(uint64_t hash, uint32_t mask) { perturb = hash; i = (uint32_t)hash & mask; j = 0; }
+    __device__ __forceinline__ uint32_t slot() const { return i + j; }
+    __device__ __forceinline__ void next(uint32_t mask) {
+        if (j < 9 && i + 9 <= mask) { j++; return; }
+        j = 0;
+        perturb >>= 5;
+        i = (uint32_t)((uint64_t)i * 5 + 1 + perturb) & mask;
+    }
+};
+// Walks on from the current slot to the first one that is empty (false) or holds the key (`eq`, true); the probe stays there.
+template <typename SlotT, typename Eq>
+__device__ __forceinline__ bool set_seek(const SlotT *tab, uint32_t mask, SetProbe &pr, Eq eq) {
+#pragma unroll 1
+    for (;;) {
+        const SlotT e = tab[pr.slot()];
+        if (e == (SlotT)~(SlotT)0) return false;
+        if (eq(e)) return true;
+        pr.next(mask);
+    }
+}
+// Ordered parallel insertion.  Every `pending` lane holds a key that is not in the table, and its probe stands on the first slot of its
+// sequence that is empty now.  Let c be the lowest pending lane whose slot a lower pending lane holds too.  Inserting the pending lanes
+// below c, in lane order, one at a time, puts each of them on the slot it stands on: slots only fill, so the slots before it on its
+// sequence are still occupied, and no lower lane of the group takes its slot (their slots all differ).  So they all commit at once;
+// `room` caps them at the insertion that makes the set grow.  Lanes from c on wait, even one that holds the lowest claim on its slot: in
+// serial order c, or a lane after it, may take that slot first.  A waiting lane whose slot was taken walks on from it (set_seek) to the
+// slot a serial insertion would reach at its turn.  The lowest pending lane always commits, so a chunk takes at most as many rounds as
+// keys.  Returns the mask of committing lanes (0: none pending).
+__device__ __forceinline__ uint32_t set_claim_round(bool pending, uint32_t slot, int lane, uint32_t room) {
+    const uint32_t pm = __ballot_sync(FULL, pending);
+    const uint32_t same = __match_any_sync(FULL, pending ? slot : 0xFFFFFFFFu) & pm;
+    const uint32_t lost = __ballot_sync(FULL, pending && (same & ((1u << lane) - 1)));
+    uint32_t cm = pm & ((lost & (0u - lost)) - 1u);  // the pending lanes below the first loser (all of them when none lost)
+#pragma unroll 1
+    while ((uint32_t)__popc(cm) > room) cm &= ~(0x80000000u >> __clz(cm));
+    return cm;
+}
+// set_table_resize: the keys of `old` re-inserted into the empty table `nt` in old slot order (set_insert_clean: no comparisons), 32 old
+// slots at a time in claim rounds.  `hash_of(key)`: the key's hash.  Ends with the warp's stores visible to every lane.
+template <typename SlotT, typename HashOf>
+__device__ __forceinline__ void set_rehash(const SlotT *old, uint32_t omask, SlotT *nt, uint32_t nmask, int lane, HashOf hash_of) {
+    constexpr SlotT EMPTY = (SlotT)~(SlotT)0;
+#pragma unroll 1
+    for (uint32_t b = 0; b <= omask; b += 32) {
+        const uint32_t s = b + lane;
+        const SlotT e = s <= omask ? old[s] : EMPTY;
+        bool pend = e != EMPTY;
+        SetProbe pr{0, 0, 0};
+        if (pend) pr.home(hash_of(e), nmask);
+#pragma unroll 1
+        for (;;) {
+            if (pend) set_seek(nt, nmask, pr, [](SlotT) { return false; });
+            const uint32_t cm = set_claim_round(pend, pr.slot(), lane, 32);
+            if (!cm) break;
+            if ((cm >> lane) & 1) { nt[pr.slot()] = e; pend = false; }
+            __syncwarp();
+        }
+    }
+}
+
 // ---- TMA 1-D bulk copies + mbarrier (PTX ISA 8.x; SASS: UBLKCP / SYNCS) ---------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {

@@ -323,7 +323,7 @@ __global__ void __launch_bounds__(64) pctc_apply_kernel(const ParamsT<CParams, S
 template <bool SEL = false>
 __global__ void __launch_bounds__(32) pctc_candidates_kernel(const ParamsT<CParams, SEL> p) {
     __shared__ uint32_t tabA[CC_TAB], tabB[512];
-    __shared__ uint64_t stg_h[32], rs_h[32];  // staged (hash, code) of the chunk's new keys / of the slots being re-inserted by a resize
+    __shared__ uint64_t stg_h[32], rs_h[32];  // staging area kept in the layout; PCTC_CANDIDATES_BODY does not use it
     __shared__ uint32_t rs_c[32];
     __shared__ uint16_t stg_c[32];
     const int lane = threadIdx.x;
