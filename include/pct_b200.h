@@ -392,14 +392,44 @@ int pct_set_items_only(pct_handle h, const int32_t *d_env, int32_t n, const void
  * All of them only enqueue work on `stream` (no host synchronisation, no allocation: CUDA-graph capturable).  On a buffered handle the
  * read-only calls (pct_query_placements*, pct_height_maps, pct_expand_items, pct_get_state, pct_get_support_graph) see the env's placed
  * boxes; pct_reset, pct_step, pct_step_envs, the _host calls, pct_set_items*, pct_reset_envs*, pct_preview_items,
- * pct_heuristic_actions* and pct_snapshot / pct_restore return PCT_ERR_STATE.  The buffered calls return PCT_ERR_STATE on a handle
- * without pct_set_buffer, and pct_buffer_step / _items / _policy_random before pct_buffer_reset. */
+ * pct_heuristic_actions* and pct_snapshot / pct_restore return PCT_ERR_STATE: pct_buffer_step_envs, pct_buffer_reset_envs and
+ * pct_buffer_snapshot / pct_buffer_restore (below) are their buffered forms.  The buffered calls return PCT_ERR_STATE on a handle
+ * without pct_set_buffer, and every one but pct_buffer_reset before pct_buffer_reset. */
 int pct_set_buffer(pct_handle h, int32_t B);
 int32_t pct_buffer_obs_len(pct_handle h);
 int pct_buffer_reset(pct_handle h, void *d_obs, pct_step_info *d_info, void *stream);
 int pct_buffer_step(pct_handle h, const int32_t *d_leaf_idx, void *d_obs, float *d_reward, uint8_t *d_done, pct_step_info *d_info, void *stream);
 int pct_buffer_items(pct_handle h, const int32_t *d_env, int32_t n, double *d_out, void *stream);
 int pct_buffer_policy_random(pct_handle h, int32_t *d_idx, uint64_t seed, const int64_t *d_t, void *stream);
+
+/* Selected envs of a buffered handle (search, evaluation quotas, asynchronous actors, early episode ends).  The selection works as in
+ * pct_step_envs: exactly one of d_env (n distinct indices; indices outside [0, n_envs) are skipped) / d_mask (n == n_envs entries, env e
+ * selected iff d_mask[e] != 0; copied before the first kernel, so the d_done of the previous call may be passed as is).  n == 0 is a no-op.
+ * Only the selected envs are read or written (observation rows, reward, done, record, buffer slots, stored leaf blocks), at a cost in
+ * proportion to the selection, and no resource is shared across envs (the buffered expansion tests placements in its own blocks, with
+ * per-(env, slot) scratch and the env's own BigScratch), so an env's trajectory does not depend on which envs step with it.
+ *
+ * pct_buffer_step_envs: pct_buffer_step for the selected envs, with the same result for each of them (select, placement, reward, done,
+ * record, refill or auto-reset, the expansion of every slot).  d_leaf_idx keeps its full size (n_envs); only selected entries are read.
+ * pct_buffer_reset_envs: env.reset() of the selected envs, mid-episode too: each gets what pct_buffer_reset gives it from the same state
+ * (the draw position is kept; under pct_set_trajectory_length it jumps to the next trajectory): slot 0 <- the reset's draw, slots 1 .. B-1
+ * <- the next B - 1 draws, every slot expanded, its rows and (d_info) its record written.
+ * Errors: PCT_ERR_INVALID for both or neither of d_env / d_mask, n < 0, a mask with n != n_envs and NULL outputs; PCT_ERR_STATE as above. */
+int pct_buffer_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, const int32_t *d_leaf_idx, void *d_obs, float *d_reward,
+                         uint8_t *d_done, pct_step_info *d_info, void *stream);
+int pct_buffer_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream);
+
+/* Buffered snapshot / restore: the contract of pct_snapshot / pct_restore (below) for buffered envs.  A buffered record is the plain
+ * record followed by the env's buffer: each slot's item as drawn, each slot's leaf count and the live rows of each slot's stored leaf
+ * block, so a flat index after a restore picks what it picked in the source env (with shuffle = 1 too).  The env's own leaf rows, which
+ * a buffered step rewrites from the chosen block before it reads them, are left out, so equal states give equal records.  Its size is fixed per handle
+ * (pct_buffer_snapshot_bytes; 0 on an unbuffered handle) and its header fingerprint combines the plain one with B: a buffered record
+ * never restores into a plain handle or one with another B, nor a plain record into a buffered handle (the env stays as it was and gets
+ * PCT_FLAG_BAD_SNAPSHOT).  pct_buffer_restore with d_obs non-NULL writes every buffered row of the restored envs (internal rows, the B
+ * leaf blocks, the B item rows): the bytes the source env's observation held.  d_buf must be 16-byte aligned. */
+int64_t pct_buffer_snapshot_bytes(pct_handle h);
+int pct_buffer_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, void *stream);
+int pct_buffer_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_t n, const void *d_buf, void *d_obs, void *stream);
 
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on

@@ -251,15 +251,16 @@ class PctBatch(object):
         """State records of envs `env_idx` (default: every env) -> (n, snapshot_bytes) uint8 CUDA tensor, filled on the current stream.
         The records hold no pointers: they can be moved to another GPU, saved and restored into any slot of a batch with the same
         configuration (restore)."""
+        return self._snapshot(env_idx, out, self.snapshot_bytes, self.L.pct_snapshot, "pct_snapshot")
+
+    def _snapshot(self, env_idx, out, B, fn, what):
         idx = self._index(env_idx, "env_idx")
         n = self.n_envs if idx is None else int(idx.numel())
-        B = self.snapshot_bytes
         if out is None:
             out = torch.empty((n, B), dtype=torch.uint8, device=self.device)
         elif out.dtype != torch.uint8 or out.device != self.device or not out.is_contiguous() or tuple(out.shape) != (n, B):
             raise PctError("snapshot out must be a contiguous (%d, %d) uint8 tensor on %s" % (n, B, self.device))
-        self._check(self.L.pct_snapshot(self.h, C.c_void_p(idx.data_ptr()) if idx is not None else None, n, C.c_void_p(out.data_ptr()),
-                                        self._stream()), "pct_snapshot")
+        self._check(fn(self.h, C.c_void_p(idx.data_ptr()) if idx is not None else None, n, C.c_void_p(out.data_ptr()), self._stream()), what)
         return out
 
     def restore(self, snap, env_idx=None, rec_idx=None, out=None, write_obs=True):
@@ -268,8 +269,11 @@ class PctBatch(object):
         rows of the restored envs into `out` (default: the batch's own observation buffer) and returns it; write_obs=False writes no rows
         (the next step then rewrites every row of the restored envs) and returns None.  A record of another configuration leaves its env
         unchanged and flags it (bad_snapshot, reported by the next step)."""
-        if snap.dtype != torch.uint8 or snap.dim() != 2 or snap.shape[1] != self.snapshot_bytes:
-            raise PctError("snapshot must be an (n, %d) uint8 tensor" % self.snapshot_bytes)
+        return self._restore(snap, env_idx, rec_idx, out, write_obs, self.snapshot_bytes, self.L.pct_restore, "pct_restore")
+
+    def _restore(self, snap, env_idx, rec_idx, out, write_obs, nbytes, fn, what):
+        if snap.dtype != torch.uint8 or snap.dim() != 2 or snap.shape[1] != nbytes:
+            raise PctError("snapshot must be an (n, %d) uint8 tensor" % nbytes)
         snap = snap.to(self.device).contiguous()
         env = self._index(env_idx, "env_idx")
         rec = self._index(rec_idx, "rec_idx")
@@ -285,9 +289,8 @@ class PctBatch(object):
             obs = self._obs if out is None else out
             if obs.dtype != self.obs_dtype or not obs.is_contiguous() or tuple(obs.shape) != (self.n_envs, self.obs_len):
                 raise PctError("restore out must be a contiguous (n_envs, obs_len) tensor of the batch's observation dtype")
-        self._check(self.L.pct_restore(self.h, C.c_void_p(env.data_ptr()) if env is not None else None,
-                                       C.c_void_p(rec.data_ptr()) if rec is not None else None, n, C.c_void_p(snap.data_ptr()),
-                                       C.c_void_p(obs.data_ptr()) if obs is not None else None, self._stream()), "pct_restore")
+        self._check(fn(self.h, C.c_void_p(env.data_ptr()) if env is not None else None, C.c_void_p(rec.data_ptr()) if rec is not None else None, n,
+                       C.c_void_p(snap.data_ptr()), C.c_void_p(obs.data_ptr()) if obs is not None else None, self._stream()), what)
         return obs
 
     # -- heuristic baselines (heuristic.py) ------------------------------------------------------------------
@@ -498,6 +501,62 @@ class PctBatch(object):
         self._check(self.L.pct_buffer_items(self.h, C.c_void_p(idx.data_ptr()) if idx is not None and n else None, n,
                                             C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_buffer_items")
         return out
+
+    # -- selected envs and snapshots of a buffered batch (include/pct_b200.h; DESIGN.md section 20) -----------------------------------
+    def _buffered(self, what):
+        if self.buffer is None:
+            raise PctError("%s: not a buffered batch (PctBatch(..., buffer=B))" % what)
+
+    def _buffer_selection(self, env_idx, mask, what):
+        self._buffered(what)
+        if env_idx is None and mask is None:
+            raise PctError("%s: pass env_idx or mask" % what)
+        return self._selection(env_idx, mask, what)
+
+    def buffer_step_envs(self, leaf_idx, env_idx=None, mask=None, out=None):
+        """step(leaf_idx) of a buffered batch for the chosen envs alone (pct_buffer_step_envs): exactly one of env_idx (distinct env indices;
+        indices outside [0, n_envs) are skipped) / mask ((n_envs,) bool / uint8 tensor, e.g. the last `done`).  leaf_idx: (n_envs,) flat leaf
+        indices j * NL + l, of which only the chosen envs' entries are read.  Returns (obs, reward, done, info), the batch's buffers (obs: `out`
+        if given), with only the chosen envs' entries written; each chosen env gets exactly what a full buffered step would give it."""
+        idx, m, n = self._buffer_selection(env_idx, mask, "buffer_step_envs")
+        leaf_idx = leaf_idx.to(torch.int32).contiguous()
+        if tuple(leaf_idx.shape) != (self.n_envs,):
+            raise PctError("leaf_idx must have shape (n_envs,)")
+        obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "buffer_step_envs out")
+        if n:
+            ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+            self._check(self.L.pct_buffer_step_envs(self.h, ptr(idx), n, ptr(m), ptr(leaf_idx), ptr(obs), ptr(self._rew), ptr(self._done),
+                                                    ptr(self._info), self._stream()), "pct_buffer_step_envs")
+        return obs, self._rew, self._done, self._info
+
+    def buffer_reset_envs(self, env_idx=None, mask=None, out=None, info=None):
+        """env.reset() of the chosen envs of a buffered batch (pct_buffer_reset_envs), mid-episode too: slot 0 takes the reset's draw and
+        slots 1 .. B-1 the next B - 1 draws, every slot is expanded.  Selection as in buffer_step_envs.  Only the chosen envs' rows of `out`
+        (default: the batch's observation buffer, returned) and of `info` (optional (n_envs, 8) int32 tensor) are written."""
+        idx, m, n = self._buffer_selection(env_idx, mask, "buffer_reset_envs")
+        obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "buffer_reset_envs out")
+        if info is not None:
+            info = self._out(info, (self.n_envs, 8), torch.int32, "buffer_reset_envs info")
+        if n:
+            ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+            self._check(self.L.pct_buffer_reset_envs(self.h, ptr(idx), n, ptr(m), ptr(obs), ptr(info), self._stream()), "pct_buffer_reset_envs")
+        return obs
+
+    @property
+    def buffer_snapshot_bytes(self):
+        """bytes of one buffered env record (fixed per batch: it depends on B)"""
+        self._buffered("buffer_snapshot_bytes")
+        return int(self.L.pct_buffer_snapshot_bytes(self.h))
+
+    def buffer_snapshot(self, env_idx=None, out=None):
+        """snapshot() of a buffered batch (pct_buffer_snapshot): the records also hold each env's buffered items and stored leaf blocks
+        -> (n, buffer_snapshot_bytes) uint8 CUDA tensor.  Restore them with buffer_restore into a batch of the same configuration and B."""
+        return self._snapshot(env_idx, out, self.buffer_snapshot_bytes, self.L.pct_buffer_snapshot, "pct_buffer_snapshot")
+
+    def buffer_restore(self, snap, env_idx=None, rec_idx=None, out=None, write_obs=True):
+        """restore() of a buffered batch (pct_buffer_restore), with the same arguments; the rows written are the buffered observation rows
+        the source env's observation held.  A plain record or one of another B leaves its env unchanged and flags it (bad_snapshot)."""
+        return self._restore(snap, env_idx, rec_idx, out, write_obs, self.buffer_snapshot_bytes, self.L.pct_buffer_restore, "pct_buffer_restore")
 
     # -- host-buffer API (what the reference's VecEnv exchanges over its pipes) --------------------------------
     def reset_host(self, obs_out):

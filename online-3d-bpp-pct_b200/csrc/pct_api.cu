@@ -920,6 +920,7 @@ int pct_set_buffer(pct_handle h, int32_t B) {
     CK(h, cudaMalloc(&h->d_buf_l, sizeof(int32_t) * n));
     CK(h, cudaMalloc(&h->d_buf_scratch, (disc ? sizeof(BufSlotD) : sizeof(BufSlotC)) * slots));
     h->buf_B = B;
+    h->buf_snap_fp = buffer_snapshot_fingerprint(h);
     return PCT_OK;
 }
 
@@ -934,24 +935,31 @@ static int check_buffered(pct_handle h, const char *what, bool after_reset) {
     return PCT_OK;
 }
 
-// select (step only), the apply kernel (reset mode without flat indices), refill + expansion, on stream st
-static int launch_buffered(pct_handle h, const int32_t *flat, void *obs, float *rew, uint8_t *done, pct_step_info *info, cudaStream_t st) {
+// select (step only), the apply kernel (reset mode without flat indices), refill + expansion, on stream st.
+// sel non-null (pct_buffer_step_envs / pct_buffer_reset_envs): every kernel over the selection; a reset of selected envs (flat == nullptr) runs
+// the reset kernel of pct_reset_envs_only in place of the apply kernel
+static int launch_buffered(pct_handle h, const int32_t *flat, void *obs, float *rew, uint8_t *done, pct_step_info *info, cudaStream_t st,
+                           const EnvSel *sel = nullptr) {
     BufParams b = buffer_params(h);
     b.flat = flat; b.done = flat ? done : nullptr; b.obs = obs; b.info = info;
     const int mode = flat ? 1 : 0;
+    const ResetParams rp = sel ? ResetParams{sel->env, sel->n, sel->mask} : ResetParams{};
+    const bool reset_sel = sel && !flat;
     if (h->cfg.domain == PCT_CONTINUOUS) {
         CParams p = continuous_params(h);
         p.leaf_idx = h->d_buf_l; p.reward = rew; p.done = done; p.info = info; p.mode = mode; p.aux = h->d_aux;
-        if (flat) CK(h, launch_buffer_select_continuous(p, b, st));
-        CK(h, launch_apply_continuous(p, h->alias_mode ? PCT_OPT_ALIAS : 0, st));
-        CK(h, launch_buffer_expand_continuous(p, b, st));
+        if (flat) CK(h, launch_buffer_select_continuous(p, b, st, sel));
+        if (reset_sel) CK(h, launch_reset_kernel_continuous(p, rp, st, sel));
+        else CK(h, launch_apply_continuous(p, h->alias_mode ? PCT_OPT_ALIAS : 0, st, sel));
+        CK(h, launch_buffer_expand_continuous(p, b, st, sel));
     } else {
         DParams p = discrete_params(h, 0, h->n_envs);
         p.leaf_idx = h->d_buf_l; p.reward = rew; p.done = done; p.info = info; p.mode = mode;
         if (h->d_aux) { p.aux = h->d_aux; p.opt = h->alias_mode ? PCT_OPT_ALIAS : 0; }
-        if (flat) CK(h, launch_buffer_select_discrete(p, b, st));
-        CK(h, launch_apply_discrete(p, st));
-        CK(h, launch_buffer_expand_discrete(p, b, st));
+        if (flat) CK(h, launch_buffer_select_discrete(p, b, st, sel));
+        if (reset_sel) CK(h, launch_reset_kernel_discrete(p, rp, st, sel));
+        else CK(h, launch_apply_discrete(p, st, sel));
+        CK(h, launch_buffer_expand_discrete(p, b, st, sel));
     }
     h->launches += flat ? 4 : 3;
     return PCT_OK;
@@ -979,6 +987,74 @@ int pct_buffer_step(pct_handle h, const int32_t *d_leaf_idx, void *d_obs, float 
     if (rc) return rc;
     CK(h, cudaSetDevice(h->device));
     return launch_buffered(h, d_leaf_idx, d_obs, d_reward, d_done, d_info, (cudaStream_t)stream);
+}
+
+int pct_buffer_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, const int32_t *d_leaf_idx, void *d_obs, float *d_reward,
+                         uint8_t *d_done, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_step_envs", false);
+    if (rc) return rc;
+    rc = check_selection(h, "pct_buffer_step_envs", d_env, n, d_mask);
+    if (rc != PCT_OK || n == 0) return rc;
+    if (!d_leaf_idx || !d_obs || !d_reward || !d_done) {
+        h->err = "pct_buffer_step_envs: d_leaf_idx, d_obs, d_reward and d_done must not be NULL";
+        return PCT_ERR_INVALID;
+    }
+    rc = check_item_source(h);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    EnvSel sel;
+    rc = resolve_selection(h, d_env, n, d_mask, st, sel);
+    if (rc) return rc;
+    return launch_buffered(h, d_leaf_idx, d_obs, d_reward, d_done, d_info, st, &sel);
+}
+
+int pct_buffer_reset_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, void *d_obs, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_reset_envs", false);
+    if (rc) return rc;
+    rc = check_selection(h, "pct_buffer_reset_envs", d_env, n, d_mask);
+    if (rc != PCT_OK || n == 0) return rc;
+    if (!d_obs) { h->err = "pct_buffer_reset_envs: d_obs is NULL"; return PCT_ERR_INVALID; }
+    rc = check_item_source(h);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    EnvSel sel;
+    rc = resolve_selection(h, d_env, n, d_mask, st, sel);
+    if (rc) return rc;
+    return launch_buffered(h, nullptr, d_obs, nullptr, nullptr, d_info, st, &sel);
+}
+
+int64_t pct_buffer_snapshot_bytes(pct_handle h) { return h && h->buf_B ? buffer_snapshot_record_bytes(h) : 0; }
+
+int pct_buffer_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_snapshot", false);
+    if (rc) return rc;
+    if (!d_buf || n < 0 || ((uintptr_t)d_buf & 15)) { h->err = "pct_buffer_snapshot: d_buf must be a 16-byte aligned device buffer and n >= 0"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_buffer_snapshot before pct_buffer_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    CK(h, cudaSetDevice(h->device));
+    CK(h, launch_buffer_snapshot(h, buffer_params(h), d_env, n, d_buf, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
+int pct_buffer_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_t n, const void *d_buf, void *d_obs, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_restore", false);
+    if (rc) return rc;
+    if (!d_buf || n < 0 || ((uintptr_t)d_buf & 15)) { h->err = "pct_buffer_restore: d_buf must be a 16-byte aligned device buffer and n >= 0"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = "pct_buffer_restore before pct_buffer_reset"; return PCT_ERR_STATE; }
+    if (n == 0) return PCT_OK;
+    CK(h, cudaSetDevice(h->device));
+    BufParams b = buffer_params(h);
+    b.obs = d_obs;
+    CK(h, launch_buffer_restore(h, b, d_env, d_rec, n, d_buf, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
 }
 
 int pct_buffer_items(pct_handle h, const int32_t *d_env, int32_t n, double *d_out, void *stream) {

@@ -16,6 +16,9 @@
 // Scratch of the expansion: the slots of one env run in different blocks, so each slot has its own candidate list and generator / shuffle
 // scratch (BufSlotD / BufSlotC); the rare many-support visits of all of them share the env's BigScratch under the env's lock (DEnvCold::lock,
 // CEnv::lock), as the pooled walks of a step do.  The env record is only read, but for the sums and the sticky flags (atomics).
+//
+// SEL (pct_buffer_step_envs / pct_buffer_reset_envs): every kernel runs over the slots of an EnvSel (SelParams, pct_kernels.h) and touches
+// the selected envs alone; the apply kernel / the reset kernel run in their own SEL instantiations.
 #include "pct_common.cuh"
 #include "pct_stability.cuh"
 #include "pct_kernels.h"
@@ -27,6 +30,7 @@
 #include "pct_cand_c.cuh"
 #include "pct_block.cuh"
 #include "pct_draw.cuh"
+#include "pct_buf_obs.cuh"
 
 // 1: one block per env takes its slots in turn (the layout of pct_expand_kernel); 0: one block per (env, slot).  A/B guard of the measurement
 // in DESIGN.md section 18, not an option of the library.
@@ -45,9 +49,14 @@ __device__ __forceinline__ void buf_decode(int d, int B, int nl, int &j, int &l)
 }
 
 // ---- select ----------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) pct_buf_select_kernel(const DParams p, const BufParams b) {
-    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (e >= p.n_envs) return;  // the whole warp
+template <bool SEL = false>
+__global__ void __launch_bounds__(256) pct_buf_select_kernel(const ParamsT<DParams, SEL> p, const BufParams b) {
+    const int slot = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    int e = slot;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, slot);
+        if (e < 0) return;  // the whole warp
+    } else if (e >= p.n_envs) return;  // the whole warp
     int j, l;
     buf_decode(b.flat[e], b.B, p.nl, j, l);
     const size_t s = (size_t)e * b.B + j;
@@ -65,9 +74,14 @@ __global__ void __launch_bounds__(256) pct_buf_select_kernel(const DParams p, co
     }
 }
 
-__global__ void __launch_bounds__(256) pctc_buf_select_kernel(const CParams p, const BufParams b) {
-    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (e >= p.n_envs) return;
+template <bool SEL = false>
+__global__ void __launch_bounds__(256) pctc_buf_select_kernel(const ParamsT<CParams, SEL> p, const BufParams b) {
+    const int slot = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    int e = slot;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, slot);
+        if (e < 0) return;
+    } else if (e >= p.n_envs) return;
     int j, l;
     buf_decode(b.flat[e], b.B, p.nl, j, l);
     const size_t s = (size_t)e * b.B + j;
@@ -114,24 +128,32 @@ __device__ __forceinline__ void buf_refill(const P &p, const BufParams &b, int e
     h.n_cand = 0;
 }
 
-__global__ void __launch_bounds__(128) pct_buf_refill_kernel(const DParams p, const BufParams b) {
-    const int e = blockIdx.x * 128 + threadIdx.x;
-    if (e >= p.n_envs) return;
+template <bool SEL = false>
+__global__ void __launch_bounds__(128) pct_buf_refill_kernel(const ParamsT<DParams, SEL> p, const BufParams b) {
+    int e = blockIdx.x * 128 + threadIdx.x;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;
+    } else if (e >= p.n_envs) return;
     DHdr h = p.hot[e].h;
     buf_refill(p, b, e, h, [&](DHdr &hh) { draw_item(p, e, hh); });
     p.hot[e].h = h;
 }
 
-__global__ void __launch_bounds__(128) pctc_buf_refill_kernel(const CParams p, const BufParams b) {
-    const int e = blockIdx.x * 128 + threadIdx.x;
-    if (e >= p.n_envs) return;
+template <bool SEL = false>
+__global__ void __launch_bounds__(128) pctc_buf_refill_kernel(const ParamsT<CParams, SEL> p, const BufParams b) {
+    int e = blockIdx.x * 128 + threadIdx.x;
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;
+    } else if (e >= p.n_envs) return;
     CHdr h = p.env[e].h;
     buf_refill(p, b, e, h, [&](CHdr &hh) { draw_item_c(p, e, hh); });
     p.env[e].h = h;
 }
 
 // ---- expand ----------------------------------------------------------------------------------------------------------------------
-// the slots of block blockIdx.x: (env, first slot, end)
+// the slots of block blockIdx.x: (env or selection slot, first slot, end)
 __device__ __forceinline__ void buf_slots(int B, int &e, int &j0, int &j1) {
     if (BUF_SLOTS_INTURN) { e = blockIdx.x; j0 = 0; j1 = B; }
     else { e = blockIdx.x / B; j0 = blockIdx.x - e * B; j1 = j0 + 1; }
@@ -143,33 +165,10 @@ __device__ __forceinline__ void buf_emit_slot(const BufParams &b, int nb, int nl
                                               int n_cand, int fl, int flags_now, int n_ems, const double sz[3], double den, Hdr *gh, int tid) {
     const int B = b.B;
     OT *o = obs + (size_t)(nb + j * nl) * 9;
-#pragma unroll 1
-    for (int f = tid; f < nl * 9; f += BUF_THREADS) {  // the leaf rows of cur_observation (write_obs / write_obs_c)
-        const int k = f / 9, col = f - k * 9;
-        OT v = 0;
-        if (k < n_leaf) {
-            if (col < 5) v = (OT)leaf[k][col];
-            else if (col == 5) v = (OT)H;
-            else if (col == 8) v = 1;
-        }
-        o[f] = v;
-    }
+    BUF_LEAF_ROWS(OT, o, leaf, n_leaf, nl, H, tid, BUF_THREADS)
     LT *dst = (LT *)b.leaf + ((size_t)e * B + j) * NL_MAX * 6;
     for (int t = tid; t < n_leaf * 6; t += BUF_THREADS) dst[t] = (&leaf[0][0])[t];
-    if (tid < 9) {  // the item row pct_set_items writes (sizes in ascending order)
-        double s0 = sz[0], s1 = sz[1], s2 = sz[2];
-        if (s1 < s0) { double t = s0; s0 = s1; s1 = t; }
-        if (s2 < s1) { double t = s1; s1 = s2; s2 = t; }
-        if (s1 < s0) { double t = s0; s0 = s1; s1 = t; }
-        const int col = tid;
-        OT v = 0;
-        if (col == 0) v = (OT)den;
-        else if (col == 3) v = (OT)s0;
-        else if (col == 4) v = (OT)s1;
-        else if (col == 5) v = (OT)s2;
-        else if (col == 8) v = 1;
-        obs[(size_t)(nb + B * nl + j) * 9 + col] = v;
-    }
+    buf_item_row<OT>(obs + (size_t)(nb + B * nl + j) * 9, sz, den, tid);
     if (tid == 0) {
         b.n_leaf[(size_t)e * B + j] = n_leaf;
         atomicAdd(&gh->n_leaf, n_leaf);
@@ -196,13 +195,17 @@ struct BufSmD {
     uint32_t wb[BUF_THREADS / 32];
 };
 
-template <typename OT, bool STAB, typename SlotT>
-__global__ void __launch_bounds__(BUF_THREADS) pct_buf_expand_kernel(const DParams p, const BufParams b) {
+template <typename OT, bool STAB, typename SlotT, bool SEL = false>
+__global__ void __launch_bounds__(BUF_THREADS) pct_buf_expand_kernel(const ParamsT<DParams, SEL> p, const BufParams b) {
     constexpr int KB = sizeof(SlotT) == 2 ? 4 : 8;
     __shared__ __align__(16) BufSmD<SlotT> s;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, B = b.B, nl = p.nl, nb = p.nb;
     int e, j0, j1;
     buf_slots(B, e, j0, j1);
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;  // the whole block
+    }
     DEnvCold *cold = p.cold + e;
     StagedD sd = stage_env_d<STAB>(s.s, p, e, false);
     const DEnvHot *hot = &s.s.hot;
@@ -210,19 +213,7 @@ __global__ void __launch_bounds__(BUF_THREADS) pct_buf_expand_kernel(const DPara
     const int n_box = h.n_box, R = p.setting == 2 ? 6 : 2;
     const RotTab *rt = &s.rt;
     OT *obs = (OT *)b.obs + (size_t)e * (size_t)((nb + B * nl + B) * 9);
-    if (j0 == 0) {
-#pragma unroll 1
-        for (int f = tid; f < nb * 9; f += BUF_THREADS) {  // the internal-node rows of write_obs
-            const int row = f / 9, col = f - row * 9;
-            OT v = 0;
-            if (row < n_box) {
-                if (col < 6) v = (OT)hot->box[row][col];
-                else if (col == 6) v = p.setting == 3 ? (OT)cold->density[row] : (OT)1;
-                else if (col == 8) v = 1;
-            } else if (row == 0 && col == 8) v = 1;
-            obs[f] = v;
-        }
-    }
+    if (j0 == 0) buf_internal_rows_d<OT, BUF_THREADS>(obs, hot, cold, nb, n_box, p.setting, tid);
 #pragma unroll 1
     for (int j = j0; j < j1; j++) {
         BufSlotD *sc = (BufSlotD *)b.scratch + (size_t)e * B + j;
@@ -285,8 +276,8 @@ __global__ void __launch_bounds__(BUF_THREADS) pct_buf_expand_kernel(const DPara
     }
 }
 
-template <typename OT, bool STAB>
-__global__ void __launch_bounds__(BUF_THREADS) pctc_buf_expand_kernel(const CParams p, const BufParams b) {
+template <typename OT, bool STAB, bool SEL = false>
+__global__ void __launch_bounds__(BUF_THREADS) pctc_buf_expand_kernel(const ParamsT<CParams, SEL> p, const BufParams b) {
     __shared__ uint32_t tabA[CC_TAB], tabB[512];
     __shared__ uint64_t stg_h[32], rs_h[32];
     __shared__ uint32_t rs_c[32];
@@ -297,6 +288,10 @@ __global__ void __launch_bounds__(BUF_THREADS) pctc_buf_expand_kernel(const CPar
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, B = b.B, nl = p.nl, NB = p.nb;
     int e, j0, j1;
     buf_slots(B, e, j0, j1);
+    if constexpr (SEL) {
+        e = sel_env(p.sel, p.n_envs, e);
+        if (e < 0) return;  // the whole block
+    }
     CEnv *env = p.env + e;
     const CHdr &h = env->h;
     const int R = p.setting == 2 ? 6 : 2, n_ems = h.n_ems, n_box = h.n_box, flags_now = h.flags;
@@ -304,20 +299,7 @@ __global__ void __launch_bounds__(BUF_THREADS) pctc_buf_expand_kernel(const CPar
     EdgePool pool{env->e_lower, env->e_next, env->e_off, env->first_in, env->last_in, env->e_st, env->e_st, h.n_edge,
                   env->poly_off, &env->poly[0][0], &env->poly[0][0], h.n_poly};
     OT *obs = (OT *)b.obs + (size_t)e * (size_t)((NB + B * nl + B) * 9);
-    if (j0 == 0) {
-#pragma unroll 1
-        for (int f = tid; f < NB * 9; f += BUF_THREADS) {  // the internal-node rows of write_obs_c
-            const int row = f / 9, col = f - row * 9;
-            double v = 0;
-            if (row < n_box) {
-                const double *bx = env->box[row];
-                if (col < 3) v = bx[col];
-                else if (col < 6) v = bx[col - 3] + bx[col];
-                else if (col == 8) v = 1;
-            } else if (row == 0 && col == 8) v = 1;
-            obs[f] = (OT)v;
-        }
-    }
+    if (j0 == 0) buf_internal_rows_c<OT, BUF_THREADS>(obs, env, NB, n_box, tid);
 #pragma unroll 1
     for (int j = j0; j < j1; j++) {
         BufSlotC *sc = (BufSlotC *)b.scratch + (size_t)e * B + j;
@@ -375,45 +357,68 @@ __global__ void pct_buf_items_kernel(const BufParams b, int n_envs, const int32_
 }
 
 // ---- launchers -------------------------------------------------------------------------------------------------------------------
-static unsigned buf_blocks(int n_envs, int B) { return BUF_SLOTS_INTURN ? (unsigned)n_envs : (unsigned)n_envs * (unsigned)B; }
+// sel non-null: the selected launches (pct_buffer_step_envs / pct_buffer_reset_envs) over sel->slots(n_envs) slots
+static unsigned buf_blocks(int slots, int B) { return BUF_SLOTS_INTURN ? (unsigned)slots : (unsigned)slots * (unsigned)B; }
 
-cudaError_t launch_buffer_select_discrete(const DParams &p, const BufParams &b, cudaStream_t st) {
-    pct_buf_select_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b);
+template <typename P>
+static SelParams<P> with_sel(const P &p, const EnvSel &sel) {
+    SelParams<P> ps;
+    static_cast<P &>(ps) = p;
+    ps.sel = sel;
+    return ps;
+}
+
+cudaError_t launch_buffer_select_discrete(const DParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel) {
+    if (sel) pct_buf_select_kernel<true><<<(sel->slots(p.n_envs) + 7) / 8, 256, 0, st>>>(with_sel(p, *sel), b);
+    else pct_buf_select_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b);
     return cudaGetLastError();
 }
 
-cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b, cudaStream_t st) {
-    pctc_buf_select_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b);
+cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel) {
+    if (sel) pctc_buf_select_kernel<true><<<(sel->slots(p.n_envs) + 7) / 8, 256, 0, st>>>(with_sel(p, *sel), b);
+    else pctc_buf_select_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b);
     return cudaGetLastError();
 }
 
-template <typename OT, bool STAB>
-static void expand_d(const DParams &p, const BufParams &b, cudaStream_t st) {
+template <typename OT, bool STAB, bool SEL>
+static void expand_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStream_t st, unsigned g) {
     const bool small = p.W <= 16 && p.L <= 16 && p.H <= 16;  // the candidate key width of the step (launch_s)
-    const unsigned g = buf_blocks(p.n_envs, b.B);
-    if (small) pct_buf_expand_kernel<OT, STAB, uint16_t><<<g, BUF_THREADS, 0, st>>>(p, b);
-    else pct_buf_expand_kernel<OT, STAB, uint32_t><<<g, BUF_THREADS, 0, st>>>(p, b);
+    if (small) pct_buf_expand_kernel<OT, STAB, uint16_t, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
+    else pct_buf_expand_kernel<OT, STAB, uint32_t, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
 }
 
-cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st) {
-    pct_buf_refill_kernel<<<(p.n_envs + 127) / 128, 128, 0, st>>>(p, b);
+template <bool SEL>
+static void buffer_expand_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
+    pct_buf_refill_kernel<SEL><<<(slots + 127) / 128, 128, 0, st>>>(p, b);
     const bool stab = p.setting != 2;
-    if (p.obs_f64) { if (stab) expand_d<double, true>(p, b, st); else expand_d<double, false>(p, b, st); }
-    else { if (stab) expand_d<float, true>(p, b, st); else expand_d<float, false>(p, b, st); }
+    const unsigned g = buf_blocks(slots, b.B);
+    if (p.obs_f64) { if (stab) expand_d<double, true, SEL>(p, b, st, g); else expand_d<double, false, SEL>(p, b, st, g); }
+    else { if (stab) expand_d<float, true, SEL>(p, b, st, g); else expand_d<float, false, SEL>(p, b, st, g); }
+}
+
+cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel) {
+    if (sel) buffer_expand_d<true>(with_sel(p, *sel), b, st, sel->slots(p.n_envs));
+    else buffer_expand_d<false>(p, b, st, p.n_envs);
     return cudaGetLastError();
 }
 
-cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st) {
-    pctc_buf_refill_kernel<<<(p.n_envs + 127) / 128, 128, 0, st>>>(p, b);
+template <bool SEL>
+static void buffer_expand_c(const ParamsT<CParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
+    pctc_buf_refill_kernel<SEL><<<(slots + 127) / 128, 128, 0, st>>>(p, b);
     const bool stab = p.setting != 2;
-    const unsigned g = buf_blocks(p.n_envs, b.B);
+    const unsigned g = buf_blocks(slots, b.B);
     if (p.obs_f64) {
-        if (stab) pctc_buf_expand_kernel<double, true><<<g, BUF_THREADS, 0, st>>>(p, b);
-        else pctc_buf_expand_kernel<double, false><<<g, BUF_THREADS, 0, st>>>(p, b);
+        if (stab) pctc_buf_expand_kernel<double, true, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
+        else pctc_buf_expand_kernel<double, false, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
     } else {
-        if (stab) pctc_buf_expand_kernel<float, true><<<g, BUF_THREADS, 0, st>>>(p, b);
-        else pctc_buf_expand_kernel<float, false><<<g, BUF_THREADS, 0, st>>>(p, b);
+        if (stab) pctc_buf_expand_kernel<float, true, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
+        else pctc_buf_expand_kernel<float, false, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
     }
+}
+
+cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel) {
+    if (sel) buffer_expand_c<true>(with_sel(p, *sel), b, st, sel->slots(p.n_envs));
+    else buffer_expand_c<false>(p, b, st, p.n_envs);
     return cudaGetLastError();
 }
 

@@ -773,17 +773,31 @@ cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemPar
     return launch_continuous(p, opt, st, false, sel);
 }
 
-cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
+cudaError_t launch_reset_kernel_continuous(const CParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
     const int slots = sel ? sel->slots(p.n_envs) : p.n_envs;
     if (sel) pctc_reset_envs_kernel<true><<<(slots + 7) / 8, 256, 0, st>>>(p, rp);
     else pctc_reset_envs_kernel<<<(slots + 7) / 8, 256, 0, st>>>(p, rp);
-    cudaError_t err = cudaGetLastError();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
+    const cudaError_t err = launch_reset_kernel_continuous(p, rp, st, sel);
     if (err != cudaSuccess) return err;
     return launch_continuous(p, opt, st, false, sel);
 }
 
-// the apply kernel alone, in plain stream order (pct_buffer_step / pct_buffer_reset)
-cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st) {
+// the apply kernel alone, in plain stream order (pct_buffer_step / pct_buffer_reset); sel: its SEL instantiation (pct_buffer_step_envs)
+cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st, const EnvSel *sel) {
+    if (sel) {
+        SelParams<CParams> ps;
+        static_cast<CParams &>(ps) = p;
+        ps.sel = *sel;
+        const int b2 = (sel->slots(p.n_envs) + 1) / 2;
+        if (p.setting != 2 && (opt & PCT_OPT_ALIAS)) pctc_apply_kernel<true, true, true><<<b2, 64, 0, st>>>(ps);
+        else if (p.setting != 2) pctc_apply_kernel<true, false, true><<<b2, 64, 0, st>>>(ps);
+        else pctc_apply_kernel<false, false, true><<<b2, 64, 0, st>>>(ps);
+        return cudaGetLastError();
+    }
     const int b2 = (p.n_envs + 1) / 2;
     if (p.setting != 2 && (opt & PCT_OPT_ALIAS)) pctc_apply_kernel<true, true><<<b2, 64, 0, st>>>(p);
     else if (p.setting != 2) pctc_apply_kernel<true, false><<<b2, 64, 0, st>>>(p);

@@ -1038,23 +1038,33 @@ cudaError_t launch_discrete(const DParams &p, cudaStream_t st, cudaEvent_t *prof
     return stab ? launch_s<float, true>(p, st, prof, apply, sel) : launch_s<float, false>(p, st, prof, apply, sel);
 }
 
-// the apply kernel alone, in plain stream order (pct_buffer_step / pct_buffer_reset: the buffered pipeline's own kernels run around it)
-template <bool STAB>
-static cudaError_t launch_apply_s(const DParams &p, cudaStream_t st) {
+// the apply kernel alone, in plain stream order (pct_buffer_step / pct_buffer_reset: the buffered pipeline's own kernels run around it);
+// SEL: over the selection's slots (pct_buffer_step_envs)
+template <bool STAB, bool SEL>
+static cudaError_t launch_apply_s(const ParamsT<DParams, SEL> &p, int slots, cudaStream_t st) {
     static bool attr_set = false;
     const size_t smem1 = (size_t)K1_SM_PER_WARP * WARPS_PER_BLOCK;
     if (!attr_set) {
-        cudaError_t err = set_smem(pct_apply_kernel<STAB, false>, smem1);
-        if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB>, smem1);
+        cudaError_t err = set_smem(pct_apply_kernel<STAB, false, SEL>, smem1);
+        if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB, SEL>, smem1);
         if (err != cudaSuccess) return err;
         attr_set = true;
     }
-    const int blocks = (p.n_envs + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-    if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
-    else pct_apply_kernel<STAB, false><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+    const int blocks = (slots + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+    if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
+    else pct_apply_kernel<STAB, false, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
     return cudaGetLastError();
 }
-cudaError_t launch_apply_discrete(const DParams &p, cudaStream_t st) { return p.setting != 2 ? launch_apply_s<true>(p, st) : launch_apply_s<false>(p, st); }
+cudaError_t launch_apply_discrete(const DParams &p, cudaStream_t st, const EnvSel *sel) {
+    if (sel) {
+        SelParams<DParams> ps;
+        static_cast<DParams &>(ps) = p;
+        ps.sel = *sel;
+        const int slots = sel->slots(p.n_envs);
+        return p.setting != 2 ? launch_apply_s<true, true>(ps, slots, st) : launch_apply_s<false, true>(ps, slots, st);
+    }
+    return p.setting != 2 ? launch_apply_s<true, false>(p, p.n_envs, st) : launch_apply_s<false, false>(p, p.n_envs, st);
+}
 
 cudaError_t launch_policy_random_discrete(const DEnvHot *hot, int n_envs, int64_t env_id_base, uint64_t seed, int64_t t, int32_t *leaf_idx,
                                           cudaStream_t st, const int64_t *t_dev) {

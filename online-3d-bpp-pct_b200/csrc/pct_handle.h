@@ -67,6 +67,7 @@ struct pct_env_batch {
     int32_t *d_buf_nleaf = nullptr;  // [n_envs][B]
     int32_t *d_buf_l = nullptr;      // [n_envs]
     void *d_buf_scratch = nullptr;   // [n_envs][B] BufSlotD / BufSlotC
+    uint64_t buf_snap_fp = 0;        // fingerprint of buffered snapshot records (snap_fp combined with B; pct_snapshot.cu)
     // staging for the host-buffer entry points
     void *d_obs = nullptr, *d_act = nullptr;
     int32_t *d_idx = nullptr;
@@ -105,6 +106,11 @@ uint64_t snapshot_fingerprint(const pct_env_batch *h);
 cudaError_t launch_snapshot(pct_env_batch *h, const int32_t *env, int n, void *buf, cudaStream_t st);
 cudaError_t launch_restore(pct_env_batch *h, const int32_t *env, const int32_t *rec, int n, const void *buf, const DParams &pd, const CParams &pc,
                            cudaStream_t st);
+// buffered records (pct_buffer_snapshot / pct_buffer_restore): b is the handle's buffer, b.obs the buffered observation to write (or nullptr)
+int64_t buffer_snapshot_record_bytes(const pct_env_batch *h);
+uint64_t buffer_snapshot_fingerprint(const pct_env_batch *h);
+cudaError_t launch_buffer_snapshot(pct_env_batch *h, const BufParams &b, const int32_t *env, int n, void *buf, cudaStream_t st);
+cudaError_t launch_buffer_restore(pct_env_batch *h, const BufParams &b, const int32_t *env, const int32_t *rec, int n, const void *buf, cudaStream_t st);
 
 // the pools of the env range [off, off + cnt): env ranges stepped concurrently (pct_step_host's staged path) own disjoint slices
 template <typename Item>

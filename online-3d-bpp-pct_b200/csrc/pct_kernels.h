@@ -337,6 +337,8 @@ struct ResetParams {
 };
 // the reset kernel, then launch_discrete(apply = false) over the batch of p (p.ready and p.order must be nullptr)
 cudaError_t launch_reset_envs_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel = nullptr);
+// the reset kernel alone (pct_buffer_reset_envs: the buffered pipeline's own kernels follow it)
+cudaError_t launch_reset_kernel_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel);
 
 // the kernel that stands in for the apply kernel of a step, exactly one non-null: the item kernel (pct_set_items) or the reset kernel
 // (pct_reset_envs).  The rest of the step's pipeline then re-expands every env of the batch.
@@ -371,6 +373,7 @@ int continuous_kernels_per_step(const CParams &p);
 cudaError_t launch_continuous(const CParams &p, int opt, cudaStream_t st, bool apply = true, const EnvSel *sel = nullptr);
 cudaError_t launch_set_items_continuous(const CParams &p, int opt, const ItemParams &ip, cudaStream_t st, const EnvSel *sel = nullptr);
 cudaError_t launch_reset_envs_continuous(const CParams &p, int opt, const ResetParams &rp, cudaStream_t st, const EnvSel *sel = nullptr);
+cudaError_t launch_reset_kernel_continuous(const CParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel);
 cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st);
 cudaError_t launch_expand_continuous(const CParams &p, const ExpandParams &x, cudaStream_t st);
 cudaError_t launch_queries_continuous(const CParams &p, const QParams &q, cudaStream_t st);
@@ -404,15 +407,16 @@ struct BufParams {
     void *obs;               // (NB + B * NL + B) * 9 values per env, the observation dtype
     pct_step_info *info;     // or nullptr
 };
-// the apply kernel alone (whole batch, plain stream order, p.order = p.ready = nullptr): pct_buffer_step / pct_buffer_reset
-cudaError_t launch_apply_discrete(const DParams &p, cudaStream_t st);
-cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st);
+// the apply kernel alone (plain stream order, p.order = p.ready = nullptr): pct_buffer_step / pct_buffer_reset; sel non-null: its SEL
+// instantiation over the selection (pct_buffer_step_envs)
+cudaError_t launch_apply_discrete(const DParams &p, cudaStream_t st, const EnvSel *sel = nullptr);
+cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st, const EnvSel *sel = nullptr);
 // the select kernel (chosen slot's item and leaf block -> the env), before the apply kernel
-cudaError_t launch_buffer_select_discrete(const DParams &p, const BufParams &b, cudaStream_t st);
-cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b, cudaStream_t st);
-// refill and expansion of every slot, the observation and the records, after the apply kernel
-cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st);
-cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st);
+cudaError_t launch_buffer_select_discrete(const DParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel = nullptr);
+cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel = nullptr);
+// refill and expansion of every slot, the observation and the records, after the apply kernel; sel non-null: of the selected envs alone
+cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel = nullptr);
+cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel = nullptr);
 cudaError_t launch_buffer_items(const BufParams &b, int n_envs, const int32_t *env, int n, double *out, cudaStream_t st);
 cudaError_t launch_buffer_policy_random(const BufParams &b, int n_envs, int nl, int64_t env_id_base, uint64_t seed, const int64_t *t_dev,
                                         int32_t *idx, cudaStream_t st);

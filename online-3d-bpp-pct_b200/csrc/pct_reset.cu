@@ -45,12 +45,16 @@ __global__ void __launch_bounds__(RESET_THREADS) pct_reset_envs_kernel(const DPa
     }
 }
 
-cudaError_t launch_reset_envs_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
+cudaError_t launch_reset_kernel_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
     constexpr int envs_per_block = RESET_THREADS / 32;
     const int slots = sel ? sel->slots(p.n_envs) : p.n_envs;
     if (sel) pct_reset_envs_kernel<true><<<(slots + envs_per_block - 1) / envs_per_block, RESET_THREADS, 0, st>>>(p, rp);
     else pct_reset_envs_kernel<<<(slots + envs_per_block - 1) / envs_per_block, RESET_THREADS, 0, st>>>(p, rp);
-    cudaError_t err = cudaGetLastError();
+    return cudaGetLastError();
+}
+
+cudaError_t launch_reset_envs_discrete(const DParams &p, const ResetParams &rp, cudaStream_t st, const EnvSel *sel) {
+    const cudaError_t err = launch_reset_kernel_discrete(p, rp, st, sel);
     if (err != cudaSuccess) return err;
     return launch_discrete(p, st, nullptr, false, sel);
 }
