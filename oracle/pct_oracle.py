@@ -39,6 +39,7 @@ def lib():
         L.pcto_get_ems.argtypes = [C.c_void_p, ip, C.c_int]
         L.pcto_get_candidates.argtypes = [C.c_void_p, ip, ip, C.c_int]
         L.pcto_get_packed.argtypes = [C.c_void_p, ip, C.c_int]
+        L.pcto_set_next.argtypes = L.pctc_set_next.argtypes = [C.c_void_p, dp, dp]
         for f in ("pcto_n_lstsq", "pcto_n_boxes", "pcto_stream_pos", "pcto_n_ems_intermediate", "pcto_n_raw_candidates", "pctc_n_ems_intermediate"):
             getattr(L, f).argtypes = [C.c_void_p]
         L.pcto_set_order6.argtypes = [C.POINTER(C.c_int64), C.c_int, ip]
@@ -141,6 +142,14 @@ class OracleDiscrete(object):
         if err:
             d["error"] = err
         return obs, rew.value, bool(done.value), d
+
+    def set_next(self, item):
+        """`env.next_box = item` (heuristic.py): item (x, y, z, density) becomes the current item on the current state -> its observation.
+        No draw is consumed; candidates(), n_raw_candidates() and ems() then describe this item"""
+        it = np.ascontiguousarray(item, dtype=np.float64).reshape(4)
+        obs = np.zeros(self.obs_len)
+        self.L.pcto_set_next(self.h, _dp(it), _dp(obs))
+        return obs
 
     def ems(self):
         buf = np.zeros((4096, 6), dtype=np.int32)
@@ -396,6 +405,13 @@ class OracleContinuous(object):
         if err:
             d["error"] = err
         return obs, rew.value, bool(done.value), d
+
+    def set_next(self, item):
+        """`env.next_box = item` (see OracleDiscrete.set_next) -> the observation of item (x, y, z, density) on the current state"""
+        it = np.ascontiguousarray(item, dtype=np.float64).reshape(4)
+        obs = np.zeros(self.obs_len)
+        self.L.pctc_set_next(self.h, _dp(it), _dp(obs))
+        return obs
 
     def ems(self):
         buf = np.zeros((1000, 6))

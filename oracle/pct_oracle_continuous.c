@@ -531,6 +531,13 @@ void pctc_reset(pctc_env *e, double *obs) {
     creator_generate(e);
     cur_observation(e, obs);
 }
+/* `env.next_box = item` and a fresh observation (heuristic.py assigns next_box and reads the env again): item4 becomes the current item on
+ * the current state; no draw is consumed */
+void pctc_set_next(pctc_env *e, const double *item4, double *obs) {
+    memcpy(e->cur_item, item4, sizeof e->cur_item);
+    e->have_item = 1;
+    cur_observation(e, obs);
+}
 
 /* C:bin3D.py:151-207 */
 int pctc_step(pctc_env *e, const double *action, int action_len, double *obs, double *reward, int *done, double *info) {

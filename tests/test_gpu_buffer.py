@@ -14,6 +14,7 @@ import pytest
 
 torch = pytest.importorskip("torch")
 from harness import ITEM_SET, case_stream, cont_case_stream, load_capacity_cases, make_stream  # noqa: E402
+from buffer_oracle import refill  # noqa: E402
 from pct_oracle import OracleContinuous, OracleDiscrete, make_continuous_stream  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -190,15 +191,17 @@ def _twin_run(P, Q, episodes=2, max_steps=600, bad_every=0, strict_flags=True):
     return t
 
 
-TWIN = [(s, c, B) for B in (3, 5) for s, c in ((1, False), (2, False), (3, False), (1, True), (3, True))]
+TWIN = [(s, c, B, 50) for B in (3, 5) for s, c in ((1, False), (2, False), (3, False), (1, True), (3, True))]
+TWIN += [(1, False, 16, 50), (3, True, 16, 50), (2, False, 16, 64)]  # BUF_MAX, and NL_MAX
 
 
-@pytest.mark.parametrize("setting,continuous,B", TWIN, ids=["%s%d-B%d" % ("c" if c else "d", s, B) for s, c, B in TWIN])
-def test_composition_twin(setting, continuous, B):
+@pytest.mark.parametrize("setting,continuous,B,nl", TWIN, ids=["%s%d-B%d%s" % ("c" if c else "d", s, B, "-nl%d" % nl if nl != 50 else "")
+                                                               for s, c, B, nl in TWIN])
+def test_composition_twin(setting, continuous, B, nl):
     n = 48
     st = _streams(n, setting, continuous, 600, seed=5)
     own = _streams(n, setting, continuous, 600, seed=6)
-    P, Q = _batch(n, setting, continuous, st, buffer=B), _batch(n, setting, continuous, own)
+    P, Q = _batch(n, setting, continuous, st, buffer=B, leaf_node_holder=nl), _batch(n, setting, continuous, own, leaf_node_holder=nl)
     P.reset(); Q.reset()
     _twin_run(P, Q, bad_every=7)
     P.close(); Q.close()
@@ -261,15 +264,7 @@ def test_items_follow_the_stream(setting, continuous, traj):
         _, _, d, _ = P.step(leaf_idx=flat)
         d = _np(d)
         for e in range(n):
-            if d[e]:
-                p0 = pos[e]
-                if traj and p0 % traj:
-                    p0 += traj - p0 % traj
-                buf[e] = st[e, [(p0 + k) % L for k in range(B)]]
-                pos[e] = p0 + B
-            else:
-                buf[e, f[e] // P.nl] = st[e, pos[e] % L]
-                pos[e] += 1
+            pos[e] = refill(buf[e], pos[e], st[e], d[e], f[e] // P.nl, traj)
         eps += d.astype(int)
         t_dev += 1
     assert eps.min() >= 2

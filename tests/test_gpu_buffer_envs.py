@@ -151,7 +151,7 @@ def _parity(A, Z, seed=0, snap_every=5, steps=None):
 # ---- 1. selection parity -----------------------------------------------------------------------------------------------------------------
 PARITY = [(s, c, B, {}) for c in (False, True) for s in ((1, 2, 3) if not c else (1, 3)) for B in (3, 5)]
 PARITY += [(1, False, 1, {}), (2, False, 3, dict(LNES="EP")), (1, False, 3, dict(shuffle=True)), (1, False, 5, dict(obs_dtype=torch.float32)),
-           (1, True, 3, dict(obs_dtype=torch.float32)), (3, False, 3, dict(traj=9))]
+           (1, True, 3, dict(obs_dtype=torch.float32)), (3, False, 3, dict(traj=9)), (1, False, 16, {}), (3, True, 16, dict(leaf_node_holder=64))]
 
 
 def _pid(c):
@@ -329,8 +329,9 @@ def _drive(X, t_dev, steps, seed=PSEED):
 
 
 @pytest.mark.parametrize("setting,continuous,B,kw", [(1, False, 3, {}), (2, False, 5, {}), (3, False, 3, dict(shuffle=True)), (1, True, 3, {}),
-                                                      (3, True, 5, dict(obs_dtype=torch.float32)), (1, False, 1, dict(LNES="CP"))],
-                         ids=["d1-B3", "d2-B5", "d3-B3-shuffle", "c1-B3", "c3-B5-f32", "d1-B1-CP"])
+                                                      (3, True, 5, dict(obs_dtype=torch.float32)), (1, False, 1, dict(LNES="CP")),
+                                                      (2, False, 16, dict(leaf_node_holder=64)), (1, True, 16, {})],
+                         ids=["d1-B3", "d2-B5", "d3-B3-shuffle", "c1-B3", "c3-B5-f32", "d1-B1-CP", "d2-B16-nl64", "c1-B16"])
 def test_snapshot_restore(setting, continuous, B, kw):
     n = 48
     st = _streams(n, setting, continuous, 900, seed=13)
@@ -361,18 +362,17 @@ def test_snapshot_restore(setting, continuous, B, kw):
         X.close()
 
 
-@pytest.mark.parametrize("continuous", [False, True], ids=["d", "c"])
-def test_fan_out(continuous):
-    """one record into many slots of another handle: identical rows; children with the same stream row and flat index step identically"""
-    n, K, B, setting = 16, 24, 3, 1
+def _fan_out(continuous, B, K=24, **kw):
+    n, setting = 16, 1
     st = _streams(n, setting, continuous, 600, seed=29)
-    P = _batch(n, setting, continuous, st, buffer=B)
+    P = _batch(n, setting, continuous, st, buffer=B, **kw)
     P.reset()
     t_dev = torch.zeros((), dtype=torch.int64, device=P.device)
     _drive(P, t_dev, 9)
     src = 5
     rec = P.buffer_snapshot(env_idx=[src])
-    S = _batch(K, setting, continuous, np.stack([st[src]] * K), buffer=B)
+    assert rec.shape == (1, P.buffer_snapshot_bytes)
+    S = _batch(K, setting, continuous, np.stack([st[src]] * K), buffer=B, **kw)
     S.reset()
     o = _np(S.buffer_restore(rec, env_idx=np.arange(K), rec_idx=np.zeros(K, dtype=np.int32)))
     assert (o == o[:1]).all() and np.array_equal(o[0].view(np.uint8), _np(P._obs[src]).view(np.uint8))
@@ -387,6 +387,17 @@ def test_fan_out(continuous):
     op, rp, _, _ = P.buffer_step_envs(f, env_idx=[src])
     assert np.array_equal(_np(op[src]).view(np.uint8), o2[0].view(np.uint8)) and float(rp[src]) == r2[0]
     P.close(); S.close()
+
+
+@pytest.mark.parametrize("continuous", [False, True], ids=["d", "c"])
+def test_fan_out(continuous):
+    """one record into many slots of another handle: identical rows; children with the same stream row and flat index step identically"""
+    _fan_out(continuous, 3)
+
+
+def test_fan_out_largest_record():
+    """the fan-out with the largest record layout: continuous (double leaf blocks), B = 16 (BUF_MAX), NL = 64 (NL_MAX)"""
+    _fan_out(True, 16, K=40, leaf_node_holder=64)
 
 
 @pytest.mark.parametrize("continuous", [False, True], ids=["d", "c"])
