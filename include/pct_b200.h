@@ -431,6 +431,31 @@ int64_t pct_buffer_snapshot_bytes(pct_handle h);
 int pct_buffer_snapshot(pct_handle h, const int32_t *d_env, int32_t n, void *d_buf, void *stream);
 int pct_buffer_restore(pct_handle h, const int32_t *d_env, const int32_t *d_rec, int32_t n, const void *d_buf, void *d_obs, void *stream);
 
+/* Item preview and item override of a buffered handle: the known future (a buffer plus k known upcoming items), chance nodes of a search
+ * (set the slot a placing step refilled to the root's real next item, or to each item of the item set), caller-given buffers (curricula,
+ * adversarial item choice, replays).  The plain pct_preview_items / pct_set_items / pct_set_items_only keep refusing buffered handles.
+ *
+ * pct_buffer_preview_items: d_out <- n x k x 4 float64 [x, y, z, density]; entry j of row i is the item env d_env[i]'s source delivers
+ * at its next draw position + j (d_env NULL: envs 0..n-1).  Entry 0 is the item the next placing step puts into the slot it empties.
+ * With B = 1, entries 0..k-1 are columns 1..k of pct_preview_items(k + 1) on a plain twin.  As in pct_preview_items: every item mode,
+ * cyclic streams, entries past a reset or trajectory jump are stale, a row outside [0, n_envs) is zeros.  Read-only.
+ *
+ * pct_buffer_set_items: d_items is n x B x 4 float64 [x, y, z, density], the layout pct_buffer_items returns (so set_items(buffer_items())
+ * is the identity).  Env d_env[i]'s B slots take row i (d_env NULL: envs 0..n-1), and every slot of that env is re-expanded against its
+ * current state.  Only the listed envs' rows of d_obs (all buffered rows) and records of d_info are written; the record: counter, sticky
+ * flags ORed with the capacity flags of the new expansions, n_leaf / n_cand summed over the slots, slot 0's n_ems, zeros for ratio /
+ * ep_reward / ep_len (the fields pct_set_items writes).  No draw is consumed: a set item stays in its slot until a step places it, and
+ * the slot then takes the consumed draw; a reset refills the whole buffer.  A buffered snapshot records the set items (same layout).
+ * Discrete sizes are truncated and clamped to [0, 255] (the range pct_set_items clamps to), and pct_buffer_items reads the converted
+ * value back; the density column is used as given (outside setting 3 the draws deliver 1).  The envs of one call must be distinct;
+ * indices outside [0, n_envs) are skipped.  The cost scales with n.
+ *
+ * Both only enqueue (no allocation: CUDA-graph capturable); n == 0 is a no-op.  Errors: PCT_ERR_STATE on an unbuffered handle or before
+ * pct_buffer_reset; PCT_ERR_INVALID for n < 0, k < 1, a NULL d_out / d_items / d_obs, or n * k * 4 / n * B * 4 past INT32_MAX. */
+int pct_buffer_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, double *d_out, void *stream);
+int pct_buffer_set_items(pct_handle h, const int32_t *d_env, int32_t n, const double *d_items, void *d_obs, pct_step_info *d_info,
+                         void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

@@ -502,6 +502,51 @@ class PctBatch(object):
                                             C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_buffer_items")
         return out
 
+    def buffer_preview_items(self, k=1, env_idx=None, out=None):
+        """The next k items of the buffered envs env_idx (default: every env) -> (n, k, 4) float64 CUDA tensor of [x, y, z, density],
+        filled on the current stream (graph-capturable, read-only).  [:, j] is the item the env's source delivers j draws from now, so
+        [:, 0] is the item the next placing step puts into the slot it empties.  A reset in between (trajectory jumps) makes the entries
+        past it stale.  Rows of an index outside [0, n_envs) are zeros.  Buffered batches only."""
+        self._buffered("buffer_preview_items")
+        k = int(k)
+        if k < 1:
+            raise PctError("buffer_preview_items: k must be >= 1")
+        idx = self._index(env_idx, "env_idx")
+        n = self.n_envs if idx is None else int(idx.numel())
+        shape = (n, k, 4)
+        out = torch.empty(shape, dtype=torch.float64, device=self.device) if out is None else self._out(out, shape, torch.float64,
+                                                                                                        "buffer_preview_items out")
+        self._check(self.L.pct_buffer_preview_items(self.h, C.c_void_p(idx.data_ptr()) if idx is not None and n else None, n, k,
+                                                    C.c_void_p(out.data_ptr()) if out.numel() else None, self._stream()), "pct_buffer_preview_items")
+        return out
+
+    def buffer_set_items(self, items, env_idx=None, out=None, info=None):
+        """Env env_idx[i] (default: env i) <- items[i] as its B buffered items, without consuming a draw, and every slot of it re-expanded
+        (pct_buffer_set_items), enqueued on the current stream (graph-capturable).  items: (n, B, 4) [x, y, z, density] per slot, the layout
+        of buffer_items(), so buffer_set_items(buffer_items()) changes nothing; discrete sizes are truncated and clamped to [0, 255].  Only the
+        listed envs' rows of `out` (default: the batch's observation buffer, returned) and of `info` (optional (n_envs, 8) int32 tensor) are
+        written.  The envs of one call must be distinct; indices outside [0, n_envs) are skipped.  A set item stays in its slot until a step
+        places it; a reset refills the whole buffer."""
+        self._buffered("buffer_set_items")
+        if not torch.is_tensor(items):
+            items = torch.as_tensor(np.asarray(items, dtype=np.float64))
+        if items.dim() != 3 or tuple(items.shape[1:]) != (self.buffer, 4):
+            raise PctError("items must have shape (n, B, 4) = (n, %d, 4): [x, y, z, density] per slot" % self.buffer)
+        n = int(items.shape[0])
+        it = items.to(device=self.device, dtype=torch.float64).contiguous()
+        idx = self._index(env_idx, "env_idx")
+        if idx is not None and int(idx.numel()) != n:
+            raise PctError("env_idx must have one entry per item row (%d)" % n)
+        if idx is None and n > self.n_envs:
+            raise PctError("%d item rows without env_idx for %d envs" % (n, self.n_envs))
+        obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "buffer_set_items out")
+        if info is not None:
+            info = self._out(info, (self.n_envs, 8), torch.int32, "buffer_set_items info")
+        if n:
+            ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+            self._check(self.L.pct_buffer_set_items(self.h, ptr(idx), n, ptr(it), ptr(obs), ptr(info), self._stream()), "pct_buffer_set_items")
+        return obs
+
     # -- selected envs and snapshots of a buffered batch (include/pct_b200.h; DESIGN.md section 20) -----------------------------------
     def _buffered(self, what):
         if self.buffer is None:

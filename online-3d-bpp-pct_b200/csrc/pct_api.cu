@@ -1070,6 +1070,53 @@ int pct_buffer_items(pct_handle h, const int32_t *d_env, int32_t n, double *d_ou
     return PCT_OK;
 }
 
+int pct_buffer_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int32_t k, double *d_out, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_preview_items", true);
+    if (rc) return rc;
+    if (n < 0 || k < 1) { h->err = "pct_buffer_preview_items: n must be >= 0 and k >= 1"; return PCT_ERR_INVALID; }
+    if ((int64_t)n * k * 4 > INT32_MAX) { h->err = "pct_buffer_preview_items: n * k * 4 overflows int32"; return PCT_ERR_INVALID; }
+    if (n == 0) return PCT_OK;
+    if (!d_out) { h->err = "pct_buffer_preview_items: d_out is NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    const ItemParams ip{d_env, n, k, nullptr, nullptr, d_out};
+    if (h->cfg.domain == PCT_CONTINUOUS) CK(h, launch_buffer_preview_continuous(continuous_params(h), ip, (cudaStream_t)stream));
+    else CK(h, launch_buffer_preview_discrete(discrete_params(h, 0, h->n_envs), ip, (cudaStream_t)stream));
+    h->launches++;
+    return PCT_OK;
+}
+
+// the set kernel in the refill kernel's place, then the expansion of every slot of the listed envs, with the parameters launch_buffered gives
+// the expansion
+int pct_buffer_set_items(pct_handle h, const int32_t *d_env, int32_t n, const double *d_items, void *d_obs, pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_set_items", true);
+    if (rc) return rc;
+    if (n < 0) { h->err = "pct_buffer_set_items: n must be >= 0"; return PCT_ERR_INVALID; }
+    if ((int64_t)n * h->buf_B * 4 > INT32_MAX) { h->err = "pct_buffer_set_items: n * B * 4 overflows int32"; return PCT_ERR_INVALID; }
+    if (n == 0) return PCT_OK;
+    if (!d_items || !d_obs) { h->err = "pct_buffer_set_items: d_items and d_obs must not be NULL"; return PCT_ERR_INVALID; }
+    CK(h, cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    EnvSel sel;
+    rc = resolve_selection(h, d_env, n, nullptr, st, sel);
+    if (rc) return rc;
+    BufParams b = buffer_params(h);
+    b.obs = d_obs; b.info = d_info;
+    if (h->cfg.domain == PCT_CONTINUOUS) {
+        CParams p = continuous_params(h);
+        p.info = d_info; p.aux = h->d_aux;
+        CK(h, launch_buffer_set_continuous(p, b, d_items, st, sel));
+    } else {
+        DParams p = discrete_params(h, 0, h->n_envs);
+        p.info = d_info;
+        if (h->d_aux) { p.aux = h->d_aux; p.opt = h->alias_mode ? PCT_OPT_ALIAS : 0; }
+        CK(h, launch_buffer_set_discrete(p, b, d_items, st, sel));
+    }
+    h->launches += 2;
+    return PCT_OK;
+}
+
 int pct_buffer_policy_random(pct_handle h, int32_t *d_idx, uint64_t seed, const int64_t *d_t, void *stream) {
     if (!h) return PCT_ERR_INVALID;
     int rc = check_buffered(h, "pct_buffer_policy_random", true);

@@ -19,6 +19,10 @@
 //
 // SEL (pct_buffer_step_envs / pct_buffer_reset_envs): every kernel runs over the slots of an EnvSel (SelParams, pct_kernels.h) and touches
 // the selected envs alone; the apply kernel / the reset kernel run in their own SEL instantiations.
+//
+// Item override (pct_buffer_set_items; DESIGN.md section 21): the set kernel writes the caller's B items of each listed env in the refill
+// kernel's place, then the SEL expansion re-expands all B slots of those envs.  Unchanged slots come out bit-identical (same state, same
+// draw position, so the same shuffle keys); all of them are re-expanded because the header's n_cand is a sum over the slots.
 #include "pct_common.cuh"
 #include "pct_stability.cuh"
 #include "pct_kernels.h"
@@ -150,6 +154,40 @@ __global__ void __launch_bounds__(128) pctc_buf_refill_kernel(const ParamsT<CPar
     CHdr h = p.env[e].h;
     buf_refill(p, b, e, h, [&](CHdr &hh) { draw_item_c(p, e, hh); });
     p.env[e].h = h;
+}
+
+// ---- set (pct_buffer_set_items) --------------------------------------------------------------------------------------------------
+// In the refill kernel's place: slot j of env d_env[i] <- item j of row i, without a draw.  Discrete sizes are truncated and clamped to
+// [0, 255] (the range pct_set_items clamps to: no container side is larger); the density is taken as given.  Zeroes the header's leaf /
+// candidate counts, which the expansion sums over the slots, and writes the record's fixed fields as pct_set_items_kernel does (counter,
+// sticky flags, zeros): the expansion adds its sums and flags.  Thread / selection slot; the row of slot i is row i.
+template <typename Hdr>
+__device__ __forceinline__ void buf_set(const BufParams &b, int e, const double *row, Hdr &h, bool disc) {
+    double *it = b.items + (size_t)e * b.B * 4;
+    for (int q = 0; q < b.B * 4; q++) {
+        const double v = row[q];
+        it[q] = disc && (q & 3) != 3 ? fmin(fmax(trunc(v), 0.0), 255.0) : v;
+    }
+    h.n_leaf = 0;
+    h.n_cand = 0;
+    if (b.info) {
+        pct_step_info info{};
+        info.counter = h.n_box;
+        info.flags = h.flags;
+        b.info[e] = info;
+    }
+}
+
+__global__ void __launch_bounds__(128) pct_buf_set_kernel(const SelParams<DParams> p, const BufParams b, const double *rows) {
+    const int i = blockIdx.x * 128 + threadIdx.x, e = sel_env(p.sel, p.n_envs, i);
+    if (e < 0) return;
+    buf_set(b, e, rows + (size_t)i * b.B * 4, p.hot[e].h, true);
+}
+
+__global__ void __launch_bounds__(128) pctc_buf_set_kernel(const SelParams<CParams> p, const BufParams b, const double *rows) {
+    const int i = blockIdx.x * 128 + threadIdx.x, e = sel_env(p.sel, p.n_envs, i);
+    if (e < 0) return;
+    buf_set(b, e, rows + (size_t)i * b.B * 4, p.env[e].h, false);
 }
 
 // ---- expand ----------------------------------------------------------------------------------------------------------------------
@@ -387,13 +425,19 @@ static void expand_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStr
     else pct_buf_expand_kernel<OT, STAB, uint32_t, SEL><<<g, BUF_THREADS, 0, st>>>(p, b);
 }
 
+// the expansion of every slot of `slots` envs / selection slots; the refill or the set kernel has run before it
 template <bool SEL>
-static void buffer_expand_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
-    pct_buf_refill_kernel<SEL><<<(slots + 127) / 128, 128, 0, st>>>(p, b);
+static void expand_slots_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
     const bool stab = p.setting != 2;
     const unsigned g = buf_blocks(slots, b.B);
     if (p.obs_f64) { if (stab) expand_d<double, true, SEL>(p, b, st, g); else expand_d<double, false, SEL>(p, b, st, g); }
     else { if (stab) expand_d<float, true, SEL>(p, b, st, g); else expand_d<float, false, SEL>(p, b, st, g); }
+}
+
+template <bool SEL>
+static void buffer_expand_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
+    pct_buf_refill_kernel<SEL><<<(slots + 127) / 128, 128, 0, st>>>(p, b);
+    expand_slots_d<SEL>(p, b, st, slots);
 }
 
 cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel) {
@@ -403,8 +447,7 @@ cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, 
 }
 
 template <bool SEL>
-static void buffer_expand_c(const ParamsT<CParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
-    pctc_buf_refill_kernel<SEL><<<(slots + 127) / 128, 128, 0, st>>>(p, b);
+static void expand_slots_c(const ParamsT<CParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
     const bool stab = p.setting != 2;
     const unsigned g = buf_blocks(slots, b.B);
     if (p.obs_f64) {
@@ -416,9 +459,29 @@ static void buffer_expand_c(const ParamsT<CParams, SEL> &p, const BufParams &b, 
     }
 }
 
+template <bool SEL>
+static void buffer_expand_c(const ParamsT<CParams, SEL> &p, const BufParams &b, cudaStream_t st, int slots) {
+    pctc_buf_refill_kernel<SEL><<<(slots + 127) / 128, 128, 0, st>>>(p, b);
+    expand_slots_c<SEL>(p, b, st, slots);
+}
+
 cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel) {
     if (sel) buffer_expand_c<true>(with_sel(p, *sel), b, st, sel->slots(p.n_envs));
     else buffer_expand_c<false>(p, b, st, p.n_envs);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_set_discrete(const DParams &p, const BufParams &b, const double *rows, cudaStream_t st, const EnvSel &sel) {
+    const SelParams<DParams> ps = with_sel(p, sel);
+    pct_buf_set_kernel<<<(sel.n + 127) / 128, 128, 0, st>>>(ps, b, rows);
+    expand_slots_d<true>(ps, b, st, sel.n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_set_continuous(const CParams &p, const BufParams &b, const double *rows, cudaStream_t st, const EnvSel &sel) {
+    const SelParams<CParams> ps = with_sel(p, sel);
+    pctc_buf_set_kernel<<<(sel.n + 127) / 128, 128, 0, st>>>(ps, b, rows);
+    expand_slots_c<true>(ps, b, st, sel.n);
     return cudaGetLastError();
 }
 

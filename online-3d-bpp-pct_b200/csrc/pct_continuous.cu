@@ -627,10 +627,12 @@ __global__ void pctc_policy_random_kernel(const CEnv *env, int n_envs, int64_t e
 }
 
 // ================= item preview / item override / per-env reset (pct_preview_items / pct_set_items / pct_reset_envs; discrete twins and notes: pct_items.cu) =================
-__global__ void __launch_bounds__(256) pctc_preview_kernel(const CParams p, const ItemParams ip) {
+// C0: the preview column of entry 0 (1: pct_buffer_preview_items, as in pct_items.cu)
+template <int C0>
+__device__ __forceinline__ void preview_entry_c(const CParams &p, const ItemParams &ip) {
     const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
     if (t >= (int64_t)ip.n * ip.k) return;
-    const int r = (int)(t / ip.k), j = (int)(t - (int64_t)r * ip.k);
+    const int r = (int)(t / ip.k), j = (int)(t - (int64_t)r * ip.k) + C0;
     const int e = ip.env ? ip.env[r] : r;
     double *o = ip.out + (size_t)t * 4;
     if (e < 0 || e >= p.n_envs) {  // not an env of this handle: a zero row
@@ -644,6 +646,9 @@ __global__ void __launch_bounds__(256) pctc_preview_kernel(const CParams p, cons
     }
     o[0] = h.next_box[0]; o[1] = h.next_box[1]; o[2] = h.next_box[2]; o[3] = h.next_den;
 }
+
+__global__ void __launch_bounds__(256) pctc_preview_kernel(const CParams p, const ItemParams ip) { preview_entry_c<0>(p, ip); }
+__global__ void __launch_bounds__(256) pctc_buf_preview_kernel(const CParams p, const ItemParams ip) { preview_entry_c<1>(p, ip); }
 
 // stands in for pctc_apply_kernel: thread t writes item t (t < n) and initialises env t's info record (t < n_envs).
 // SEL (pct_set_items_only): thread t writes item t and the info record of its env, nothing else.
@@ -808,6 +813,12 @@ cudaError_t launch_apply_continuous(const CParams &p, int opt, cudaStream_t st, 
 cudaError_t launch_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st) {
     const int64_t n = (int64_t)ip.n * ip.k;
     pctc_preview_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, ip);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st) {
+    const int64_t n = (int64_t)ip.n * ip.k;
+    pctc_buf_preview_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, ip);
     return cudaGetLastError();
 }
 

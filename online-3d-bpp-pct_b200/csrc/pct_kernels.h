@@ -417,6 +417,13 @@ cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b
 // refill and expansion of every slot, the observation and the records, after the apply kernel; sel non-null: of the selected envs alone
 cudaError_t launch_buffer_expand_discrete(const DParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel = nullptr);
 cudaError_t launch_buffer_expand_continuous(const CParams &p, const BufParams &b, cudaStream_t st, const EnvSel *sel = nullptr);
+// item override (pct_buffer_set_items): the set kernel (rows: sel.n x B x 4 float64, row i for selection slot i) in the refill kernel's
+// place, then the expansion of every slot of the selected envs
+cudaError_t launch_buffer_set_discrete(const DParams &p, const BufParams &b, const double *rows, cudaStream_t st, const EnvSel &sel);
+cudaError_t launch_buffer_set_continuous(const CParams &p, const BufParams &b, const double *rows, cudaStream_t st, const EnvSel &sel);
+// item preview (pct_buffer_preview_items; pct_items.cu / pct_continuous.cu): entry j of row r is the draw at the env's draw position + j
+cudaError_t launch_buffer_preview_discrete(const DParams &p, const ItemParams &ip, cudaStream_t st);
+cudaError_t launch_buffer_preview_continuous(const CParams &p, const ItemParams &ip, cudaStream_t st);
 cudaError_t launch_buffer_items(const BufParams &b, int n_envs, const int32_t *env, int n, double *out, cudaStream_t st);
 cudaError_t launch_buffer_policy_random(const BufParams &b, int n_envs, int nl, int64_t env_id_base, uint64_t seed, const int64_t *t_dev,
                                         int32_t *idx, cudaStream_t st);
