@@ -456,6 +456,34 @@ int pct_buffer_preview_items(pct_handle h, const int32_t *d_env, int32_t n, int3
 int pct_buffer_set_items(pct_handle h, const int32_t *d_env, int32_t n, const double *d_items, void *d_obs, pct_step_info *d_info,
                          void *stream);
 
+/* Heuristic baselines of a buffered handle: the baseline picks the buffered item and its placement.  Let choice_j be what
+ * pct_heuristic_actions (_f64) returns for the env after pct_set_items(item j) on a plain handle: the plain baseline run for slot j's item on
+ * the env's current state, with the same enumeration, scores and tie rules.  Then
+ *   LSAH, BR, MACS, DBL, HM: the slot whose choice_j has the best score in the baseline's own direction (the least for LSAH, DBL and HM,
+ *     the greatest for BR and MACS), ties to the lowest slot;
+ *   OnlineBPH: the slot whose first feasible placement has the lowest rank of its EMS in the (z, y, x) order, ties to the lowest slot: the
+ *     first feasible candidate in the order (EMS rank, slot, rotation);
+ *   RANDOM: a slot drawn uniformly among the slots with a feasible placement, with rnd(seed ^ 0xB0FF510F, env_id_base+e, t), then that
+ *     slot's plain choice, drawn with rnd(seed, env_id_base+e, t) as the plain call draws it;
+ *   no slot with a feasible placement: slot 0 and the plain call's "no placement" row, which ends the episode at the step.
+ * At B = 1 every rule is the plain baseline.  d_slots[e] <- the slot, d_rows[e] <- choice_slot (float32 N x 9 / float64 N x 9 for the
+ * continuous domain, LSAH / OnlineBPH / BR only).  LSAH's footprint (per env in the handle) takes the chosen placement only.
+ *
+ * pct_buffer_step_rows: steps every env by slot d_slots[e] and action row e of d_rows (float32 or, rows_f64 != 0, float64; N x 9): exactly
+ * pct_set_items(item d_slots[e]) followed by pct_step(row e) on a plain handle, with pct_step's row rules (LeafNode2Action, the continuous
+ * 1e-6 tolerance, PCT_FLAG_BAD_ACTION), then the refill and expansion of pct_buffer_step: the placed item's slot takes the draw the step
+ * consumed, a finished episode refills every slot.  A slot outside [0, B) is slot 0 with the zero action, as pct_buffer_step treats a
+ * flat index outside [0, B * NL).  Results as pct_buffer_step.
+ *
+ * All three only enqueue (no allocation: CUDA-graph capturable).  Errors: PCT_ERR_STATE on an unbuffered handle, before
+ * pct_buffer_reset, and for PCT_H_BR without pct_set_item_set; PCT_ERR_INVALID for an unknown heuristic, the other domain's call, a
+ * baseline the continuous domain does not allow, or a NULL output / input buffer.  The plain pct_heuristic_actions* keep refusing a
+ * buffered handle. */
+int pct_buffer_heuristic_actions(pct_handle h, int32_t heuristic, int32_t *d_slots, float *d_rows, uint64_t seed, int64_t t, void *stream);
+int pct_buffer_heuristic_actions_f64(pct_handle h, int32_t heuristic, int32_t *d_slots, double *d_rows, void *stream);
+int pct_buffer_step_rows(pct_handle h, const int32_t *d_slots, const void *d_rows, int32_t rows_f64, void *d_obs, float *d_reward, uint8_t *d_done,
+                         pct_step_info *d_info, void *stream);
+
 /* Snapshot / restore of env states on the device: branch an env (lookahead, beam search, Monte Carlo rollouts), copy it into other
  * slots, move it to another handle or GPU, or checkpoint a batch mid-episode.  Like pct_step, both calls only enqueue kernels on
  * `stream`: no host synchronisation, no allocation (CUDA-graph capturable).

@@ -69,7 +69,8 @@ EXPORTS = ["pct_create", "pct_destroy", "pct_last_error", "pct_set_item_set", "p
            "pct_preview_items", "pct_set_items", "pct_expand_items", "pct_reset_envs", "pct_get_support_graph",
            "pct_step_envs", "pct_reset_envs_only", "pct_set_items_only", "pct_set_buffer", "pct_buffer_obs_len", "pct_buffer_reset",
            "pct_buffer_step", "pct_buffer_items", "pct_buffer_policy_random", "pct_buffer_step_envs", "pct_buffer_reset_envs",
-           "pct_buffer_snapshot_bytes", "pct_buffer_snapshot", "pct_buffer_restore", "pct_buffer_preview_items", "pct_buffer_set_items"]
+           "pct_buffer_snapshot_bytes", "pct_buffer_snapshot", "pct_buffer_restore", "pct_buffer_preview_items", "pct_buffer_set_items",
+           "pct_buffer_heuristic_actions", "pct_buffer_heuristic_actions_f64", "pct_buffer_step_rows"]
 
 
 def build(verbose=False):
@@ -148,5 +149,8 @@ def lib():
     L.pct_buffer_restore.argtypes = [vp, vp, vp, i32, vp, vp, vp]
     L.pct_buffer_preview_items.argtypes = [vp, vp, i32, i32, vp, vp]
     L.pct_buffer_set_items.argtypes = [vp, vp, i32, vp, vp, vp, vp]
+    L.pct_buffer_heuristic_actions.argtypes = [vp, i32, vp, vp, u64, i64, vp]
+    L.pct_buffer_heuristic_actions_f64.argtypes = [vp, i32, vp, vp, vp]
+    L.pct_buffer_step_rows.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp]
     _lib = L
     return L

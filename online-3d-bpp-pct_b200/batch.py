@@ -547,6 +547,51 @@ class PctBatch(object):
             self._check(self.L.pct_buffer_set_items(self.h, ptr(idx), n, ptr(it), ptr(obs), ptr(info), self._stream()), "pct_buffer_set_items")
         return obs
 
+    # -- heuristic baselines of a buffered batch (include/pct_b200.h; DESIGN.md section 22) -------------------------------------------
+    def buffer_heuristic_actions(self, name, seed=0, t=0, out=None):
+        """(slots (n_envs,) int32, rows (n_envs, 9)) CUDA tensors: the buffered item and the placement the baseline `name` picks for every env
+        (pct_buffer_heuristic_actions / _f64): the slot whose plain choice scores best (OnlineBPH: the lowest EMS rank; RANDOM: a uniform
+        slot among those with a placement), and that choice's row.  At B = 1 it is heuristic_actions.  Rows are float32, float64 in the
+        continuous domain (LSAH / OnlineBPH / BR only).  Feed both to buffer_step_rows.  out: optional (slots, rows) tensors to fill.
+        Without `out`, the batch's own buffers, rewritten by the next call."""
+        self._buffered("buffer_heuristic_actions")
+        if name not in _lib.HEURISTIC_CODES:
+            raise PctError("unknown heuristic %r" % (name,))
+        rdt = torch.float64 if self.continuous else torch.float32
+        if out is None:
+            if getattr(self, "_bh_out", None) is None:
+                self._bh_out = (torch.zeros((self.n_envs,), dtype=torch.int32, device=self.device),
+                                torch.zeros((self.n_envs, 9), dtype=rdt, device=self.device))
+            out = self._bh_out
+        slots = self._out(out[0], (self.n_envs,), torch.int32, "buffer_heuristic_actions slots")
+        rows = self._out(out[1], (self.n_envs, 9), rdt, "buffer_heuristic_actions rows")
+        code = _lib.HEURISTIC_CODES[name]
+        if self.continuous:
+            self._check(self.L.pct_buffer_heuristic_actions_f64(self.h, code, C.c_void_p(slots.data_ptr()), C.c_void_p(rows.data_ptr()),
+                                                                self._stream()), "pct_buffer_heuristic_actions_f64")
+        else:
+            self._check(self.L.pct_buffer_heuristic_actions(self.h, code, C.c_void_p(slots.data_ptr()), C.c_void_p(rows.data_ptr()),
+                                                            int(seed) & ((1 << 64) - 1), int(t), self._stream()), "pct_buffer_heuristic_actions")
+        return slots, rows
+
+    def buffer_step_rows(self, slots, rows, out=None):
+        """Step every env of a buffered batch by buffered item slots[e] placed by action row rows[e] (pct_buffer_step_rows): exactly
+        set_items(item slots[e]) + step(actions=rows) on a plain batch, then the buffer's refill and expansion.  A slot outside [0, B) is slot
+        0 with the zero action.  slots: (n_envs,) integer; rows: (n_envs, 9) float32 / float64 CUDA tensors.  Returns (obs, reward, done,
+        info) as step() does."""
+        self._buffered("buffer_step_rows")
+        slots = slots.to(device=self.device, dtype=torch.int32).contiguous()
+        if rows.dtype not in (torch.float32, torch.float64):
+            rows = rows.float()
+        rows = rows.to(self.device).contiguous()
+        if tuple(slots.shape) != (self.n_envs,) or tuple(rows.shape) != (self.n_envs, 9):
+            raise PctError("slots must have shape (n_envs,) and rows (n_envs, 9)")
+        obs = self._obs if out is None else self._out(out, (self.n_envs, self.obs_len), self.obs_dtype, "buffer_step_rows out")
+        self._check(self.L.pct_buffer_step_rows(self.h, C.c_void_p(slots.data_ptr()), C.c_void_p(rows.data_ptr()), int(rows.dtype == torch.float64),
+                                                C.c_void_p(obs.data_ptr()), C.c_void_p(self._rew.data_ptr()), C.c_void_p(self._done.data_ptr()),
+                                                C.c_void_p(self._info.data_ptr()), self._stream()), "pct_buffer_step_rows")
+        return obs, self._rew, self._done, self._info
+
     # -- selected envs and snapshots of a buffered batch (include/pct_b200.h; DESIGN.md section 20) -----------------------------------
     def _buffered(self, what):
         if self.buffer is None:

@@ -207,7 +207,10 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
         if (e == cudaSuccess) e = cudaMemset(h->d_cold, 0, sizeof(DEnvCold) * (size_t)n_envs);
         // HM / MACS / RANDOM on a bin wider than 32 cells run with dynamic shared memory: raise its limit here, so that
         // pct_heuristic_actions stays enqueue-only (capturable)
-        if (e == cudaSuccess && (cfg->container_size[0] > HEUR_SIDE_MAX || cfg->container_size[1] > HEUR_SIDE_MAX)) e = prepare_heuristic_big();
+        if (e == cudaSuccess && (cfg->container_size[0] > HEUR_SIDE_MAX || cfg->container_size[1] > HEUR_SIDE_MAX)) {
+            e = prepare_heuristic_big();
+            if (e == cudaSuccess) e = prepare_buffer_heuristic_big();
+        }
     } else {
         if (e == cudaSuccess) e = cudaMalloc(&h->d_cenv, sizeof(CEnv) * (size_t)n_envs);
         if (e == cudaSuccess) e = cudaMemset(h->d_cenv, 0, sizeof(CEnv) * (size_t)n_envs);
@@ -246,7 +249,7 @@ void pct_destroy(pct_handle h) {
     cudaFree(h->d_hstate); cudaFree(h->d_hstate_c); cudaFree(h->d_query_c); cudaFree(h->d_query); cudaFree(h->d_aux);
     cudaFree(h->d_ready); cudaFree(h->d_sel_mask);
     cudaFree(h->d_hot); cudaFree(h->d_cold); cudaFree(h->d_item_set); cudaFree(h->d_stream);
-    cudaFree(h->d_buf_items); cudaFree(h->d_buf_leaf); cudaFree(h->d_buf_nleaf); cudaFree(h->d_buf_l); cudaFree(h->d_buf_scratch);
+    cudaFree(h->d_buf_items); cudaFree(h->d_buf_leaf); cudaFree(h->d_buf_nleaf); cudaFree(h->d_buf_l); cudaFree(h->d_buf_scratch); cudaFree(h->d_buf_rows);
     cudaFree(h->d_obs); cudaFree(h->d_act); cudaFree(h->d_idx); cudaFree(h->d_rew); cudaFree(h->d_done); cudaFree(h->d_info);
     for (cudaEvent_t ev : h->prof_ev) if (ev) cudaEventDestroy(ev);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
@@ -908,8 +911,9 @@ int pct_set_buffer(pct_handle h, int32_t B) {
     if (B < 1 || B > BUF_MAX) { h->err = "pct_set_buffer: B must be in [1, 16]"; return PCT_ERR_INVALID; }
     if (h->cfg.no_auto_reset) { h->err = "pct_set_buffer: buffered envs auto-reset (no_auto_reset = 1 is not supported)"; return PCT_ERR_INVALID; }
     CK(h, cudaSetDevice(h->device));
-    cudaFree(h->d_buf_items); cudaFree(h->d_buf_leaf); cudaFree(h->d_buf_nleaf); cudaFree(h->d_buf_l); cudaFree(h->d_buf_scratch);
+    cudaFree(h->d_buf_items); cudaFree(h->d_buf_leaf); cudaFree(h->d_buf_nleaf); cudaFree(h->d_buf_l); cudaFree(h->d_buf_scratch); cudaFree(h->d_buf_rows);
     h->d_buf_items = nullptr; h->d_buf_leaf = nullptr; h->d_buf_nleaf = nullptr; h->d_buf_l = nullptr; h->d_buf_scratch = nullptr;
+    h->d_buf_rows = nullptr;
     h->buf_B = 0;
     const bool disc = h->cfg.domain == PCT_DISCRETE;
     const size_t n = (size_t)h->n_envs, slots = n * (size_t)B;
@@ -919,6 +923,7 @@ int pct_set_buffer(pct_handle h, int32_t B) {
     CK(h, cudaMemset(h->d_buf_nleaf, 0, sizeof(int32_t) * slots));
     CK(h, cudaMalloc(&h->d_buf_l, sizeof(int32_t) * n));
     CK(h, cudaMalloc(&h->d_buf_scratch, (disc ? sizeof(BufSlotD) : sizeof(BufSlotC)) * slots));
+    CK(h, cudaMalloc(&h->d_buf_rows, sizeof(double) * 9 * n));
     h->buf_B = B;
     h->buf_snap_fp = buffer_snapshot_fingerprint(h);
     return PCT_OK;
@@ -938,9 +943,18 @@ static int check_buffered(pct_handle h, const char *what, bool after_reset) {
 // select (step only), the apply kernel (reset mode without flat indices), refill + expansion, on stream st.
 // sel non-null (pct_buffer_step_envs / pct_buffer_reset_envs): every kernel over the selection; a reset of selected envs (flat == nullptr) runs
 // the reset kernel of pct_reset_envs_only in place of the apply kernel
+// rows non-null (pct_buffer_step_rows; flat == nullptr, whole batch): the row select kernel in the select kernel's place, the apply kernel on the
+// float64 rows it writes, the refill on the slots it names in d_buf_l
+struct BufRows {
+    const int32_t *slots;
+    const void *rows;
+    int f64;
+};
+
 static int launch_buffered(pct_handle h, const int32_t *flat, void *obs, float *rew, uint8_t *done, pct_step_info *info, cudaStream_t st,
-                           const EnvSel *sel = nullptr) {
+                           const EnvSel *sel = nullptr, const BufRows *rows = nullptr) {
     BufParams b = buffer_params(h);
+    if (rows) flat = h->d_buf_l;
     b.flat = flat; b.done = flat ? done : nullptr; b.obs = obs; b.info = info;
     const int mode = flat ? 1 : 0;
     const ResetParams rp = sel ? ResetParams{sel->env, sel->n, sel->mask} : ResetParams{};
@@ -948,7 +962,10 @@ static int launch_buffered(pct_handle h, const int32_t *flat, void *obs, float *
     if (h->cfg.domain == PCT_CONTINUOUS) {
         CParams p = continuous_params(h);
         p.leaf_idx = h->d_buf_l; p.reward = rew; p.done = done; p.info = info; p.mode = mode; p.aux = h->d_aux;
-        if (flat) CK(h, launch_buffer_select_continuous(p, b, st, sel));
+        if (rows) {
+            CK(h, launch_buffer_select_rows_continuous(p, b, rows->slots, rows->rows, rows->f64, h->d_buf_rows, st));
+            p.leaf_idx = nullptr; p.actions = h->d_buf_rows; p.action_f64 = 1;
+        } else if (flat) CK(h, launch_buffer_select_continuous(p, b, st, sel));
         if (reset_sel) CK(h, launch_reset_kernel_continuous(p, rp, st, sel));
         else CK(h, launch_apply_continuous(p, h->alias_mode ? PCT_OPT_ALIAS : 0, st, sel));
         CK(h, launch_buffer_expand_continuous(p, b, st, sel));
@@ -956,7 +973,10 @@ static int launch_buffered(pct_handle h, const int32_t *flat, void *obs, float *
         DParams p = discrete_params(h, 0, h->n_envs);
         p.leaf_idx = h->d_buf_l; p.reward = rew; p.done = done; p.info = info; p.mode = mode;
         if (h->d_aux) { p.aux = h->d_aux; p.opt = h->alias_mode ? PCT_OPT_ALIAS : 0; }
-        if (flat) CK(h, launch_buffer_select_discrete(p, b, st, sel));
+        if (rows) {
+            CK(h, launch_buffer_select_rows_discrete(p, b, rows->slots, rows->rows, rows->f64, h->d_buf_rows, st));
+            p.leaf_idx = nullptr; p.actions = h->d_buf_rows; p.action_f64 = 1;
+        } else if (flat) CK(h, launch_buffer_select_discrete(p, b, st, sel));
         if (reset_sel) CK(h, launch_reset_kernel_discrete(p, rp, st, sel));
         else CK(h, launch_apply_discrete(p, st, sel));
         CK(h, launch_buffer_expand_discrete(p, b, st, sel));
@@ -987,6 +1007,66 @@ int pct_buffer_step(pct_handle h, const int32_t *d_leaf_idx, void *d_obs, float 
     if (rc) return rc;
     CK(h, cudaSetDevice(h->device));
     return launch_buffered(h, d_leaf_idx, d_obs, d_reward, d_done, d_info, (cudaStream_t)stream);
+}
+
+int pct_buffer_step_rows(pct_handle h, const int32_t *d_slots, const void *d_rows, int32_t rows_f64, void *d_obs, float *d_reward, uint8_t *d_done,
+                         pct_step_info *d_info, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffered(h, "pct_buffer_step_rows", true);
+    if (rc) return rc;
+    if (!d_slots || !d_rows || !d_obs || !d_reward || !d_done) {
+        h->err = "pct_buffer_step_rows: d_slots, d_rows, d_obs, d_reward and d_done must not be NULL";
+        return PCT_ERR_INVALID;
+    }
+    rc = check_item_source(h);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    const BufRows rows{d_slots, d_rows, rows_f64 ? 1 : 0};
+    return launch_buffered(h, nullptr, d_obs, d_reward, d_done, d_info, (cudaStream_t)stream, nullptr, &rows);
+}
+
+// the checks of both pct_buffer_heuristic_actions calls, in the order of the plain calls' checks
+static int check_buffer_heuristic(pct_handle h, const char *what, int32_t heuristic, const int32_t *d_slots, const void *d_rows, bool cont) {
+    if (heuristic < PCT_H_LSAH || heuristic > PCT_H_RANDOM) { h->err = std::string(what) + ": unknown heuristic"; return PCT_ERR_INVALID; }
+    int rc = check_buffered(h, what, false);
+    if (rc) return rc;
+    if ((h->cfg.domain == PCT_CONTINUOUS) != cont) {
+        h->err = std::string(what) + (cont ? ": continuous domain only (discrete: pct_buffer_heuristic_actions)"
+                                           : ": discrete domain only (continuous: pct_buffer_heuristic_actions_f64)");
+        return PCT_ERR_INVALID;
+    }
+    if (cont && heuristic != PCT_H_LSAH && heuristic != PCT_H_ONLINEBPH && heuristic != PCT_H_BR) {  // tools.py:217-218
+        h->err = "only LSAH, OnlineBPH, and BR allowed for continuous environment";
+        return PCT_ERR_INVALID;
+    }
+    if (!d_slots || !d_rows) { h->err = std::string(what) + ": d_slots and d_rows must not be NULL"; return PCT_ERR_INVALID; }
+    if (!h->did_reset) { h->err = std::string(what) + " before pct_buffer_reset"; return PCT_ERR_STATE; }
+    if (heuristic == PCT_H_BR && !h->d_item_set) { h->err = "PCT_H_BR scores an EMS by the item types that fit: call pct_set_item_set"; return PCT_ERR_STATE; }
+    return PCT_OK;
+}
+
+int pct_buffer_heuristic_actions(pct_handle h, int32_t heuristic, int32_t *d_slots, float *d_rows, uint64_t seed, int64_t t, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffer_heuristic(h, "pct_buffer_heuristic_actions", heuristic, d_slots, d_rows, false);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    HParams hp{};
+    hp.code = heuristic; hp.rows = d_rows; hp.hstate = h->d_hstate; hp.seed = seed; hp.t = t;
+    CK(h, launch_buffer_heuristic_discrete(discrete_params(h, 0, h->n_envs), hp, buffer_params(h), d_slots, (cudaStream_t)stream));
+    h->launches += 2;
+    return PCT_OK;
+}
+
+int pct_buffer_heuristic_actions_f64(pct_handle h, int32_t heuristic, int32_t *d_slots, double *d_rows, void *stream) {
+    if (!h) return PCT_ERR_INVALID;
+    int rc = check_buffer_heuristic(h, "pct_buffer_heuristic_actions_f64", heuristic, d_slots, d_rows, true);
+    if (rc) return rc;
+    CK(h, cudaSetDevice(h->device));
+    HParamsC hp{};
+    hp.code = heuristic; hp.rows = d_rows; hp.hstate = h->d_hstate_c;
+    CK(h, launch_buffer_heuristic_continuous(continuous_params(h), hp, buffer_params(h), d_slots, (cudaStream_t)stream));
+    h->launches += 2;
+    return PCT_OK;
 }
 
 int pct_buffer_step_envs(pct_handle h, const int32_t *d_env, int32_t n, const uint8_t *d_mask, const int32_t *d_leaf_idx, void *d_obs, float *d_reward,

@@ -23,6 +23,11 @@
 // Item override (pct_buffer_set_items; DESIGN.md section 21): the set kernel writes the caller's B items of each listed env in the refill
 // kernel's place, then the SEL expansion re-expands all B slots of those envs.  Unchanged slots come out bit-identical (same state, same
 // draw position, so the same shuffle keys); all of them are re-expanded because the header's n_cand is a sum over the slots.
+//
+// Heuristic baselines (pct_buffer_heuristic_actions*; DESIGN.md section 22): the plain baselines' selection (heur_select / heur_select_c) in one
+// block per (env, slot) on the slot's item, a per-slot result in the slot's scratch, and a pick kernel per env.  pct_buffer_step_rows runs the
+// row select kernel in the select kernel's place; apply, refill and expansion are the step's.  In this translation unit, beside the expansion,
+// because the selections share the env's BigScratch under the env's lock as the expansion does.
 #include "pct_common.cuh"
 #include "pct_stability.cuh"
 #include "pct_kernels.h"
@@ -35,6 +40,10 @@
 #include "pct_block.cuh"
 #include "pct_draw.cuh"
 #include "pct_buf_obs.cuh"
+// the heuristic selections of pct_buffer_heuristic_actions*: a block of BUF_THREADS threads per (env, slot)
+namespace pct { constexpr int FEAS_THREADS = 64; }
+#include "pct_heur_select.cuh"
+#include "pct_heur_select_c.cuh"
 
 // 1: one block per env takes its slots in turn (the layout of pct_expand_kernel); 0: one block per (env, slot).  A/B guard of the measurement
 // in DESIGN.md section 18, not an option of the library.
@@ -100,6 +109,61 @@ __global__ void __launch_bounds__(256) pctc_buf_select_kernel(const ParamsT<CPar
         ev->h.next_den = it[3];
         ev->h.n_leaf = n;
         b.l[e] = l;
+    }
+}
+
+// ---- select by slot and row (pct_buffer_step_rows) ----------------------------------------------------------------------------------
+// Warp / env, as the select kernel: slot slots[e] (outside [0, B): slot 0) becomes the env's current item and leaf list.  The caller's row
+// goes to the apply kernel as a float64 row in `act` (a float32 row converts exactly, as the apply kernel converts it; outside: the zero
+// action), and b.l[e] = slot * NL, a flat index the refill kernel decodes back into the slot.
+__device__ __forceinline__ int buf_take_row(const BufParams &b, int e, int nl, const int32_t *slots, const void *rows, int rows_f64, double *act,
+                                            int lane) {
+    const int s = slots[e];
+    const bool in = s >= 0 && s < b.B;
+    const int j = in ? s : 0;
+    if (lane < 9) {
+        const size_t q = (size_t)e * 9 + lane;
+        act[q] = !in ? 0.0 : rows_f64 ? ((const double *)rows)[q] : (double)((const float *)rows)[q];
+    }
+    if (lane == 0) b.l[e] = j * nl;
+    return j;
+}
+
+__global__ void __launch_bounds__(256) pct_buf_select_rows_kernel(const DParams p, const BufParams b, const int32_t *slots, const void *rows,
+                                                                  int rows_f64, double *act) {
+    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (e >= p.n_envs) return;  // the whole warp
+    const int j = buf_take_row(b, e, p.nl, slots, rows, rows_f64, act, lane);
+    const size_t s = (size_t)e * b.B + j;
+    const int n = b.n_leaf[s];
+    const int16_t *src = (const int16_t *)b.leaf + s * NL_MAX * 6;
+    int16_t *dst = &p.cold[e].leaf[0][0];
+    for (int t = lane; t < n * 6; t += 32) dst[t] = src[t];
+    if (lane == 0) {
+        DHdr &h = p.hot[e].h;
+        const double *it = b.items + s * 4;
+        h.next_box[0] = (int)it[0]; h.next_box[1] = (int)it[1]; h.next_box[2] = (int)it[2];
+        h.next_den = it[3];
+        h.n_leaf = n;
+    }
+}
+
+__global__ void __launch_bounds__(256) pctc_buf_select_rows_kernel(const CParams p, const BufParams b, const int32_t *slots, const void *rows,
+                                                                   int rows_f64, double *act) {
+    const int e = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (e >= p.n_envs) return;
+    const int j = buf_take_row(b, e, p.nl, slots, rows, rows_f64, act, lane);
+    const size_t s = (size_t)e * b.B + j;
+    const int n = b.n_leaf[s];
+    const double *src = (const double *)b.leaf + s * NL_MAX * 6;
+    CEnv *ev = p.env + e;
+    double *dst = &ev->leaf[0][0];
+    for (int t = lane; t < n * 6; t += 32) dst[t] = src[t];
+    if (lane == 0) {
+        const double *it = b.items + s * 4;
+        ev->h.next_box[0] = it[0]; ev->h.next_box[1] = it[1]; ev->h.next_box[2] = it[2];
+        ev->h.next_den = it[3];
+        ev->h.n_leaf = n;
     }
 }
 
@@ -418,6 +482,18 @@ cudaError_t launch_buffer_select_continuous(const CParams &p, const BufParams &b
     return cudaGetLastError();
 }
 
+cudaError_t launch_buffer_select_rows_discrete(const DParams &p, const BufParams &b, const int32_t *slots, const void *rows, int rows_f64, double *act,
+                                               cudaStream_t st) {
+    pct_buf_select_rows_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b, slots, rows, rows_f64, act);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_select_rows_continuous(const CParams &p, const BufParams &b, const int32_t *slots, const void *rows, int rows_f64,
+                                                 double *act, cudaStream_t st) {
+    pctc_buf_select_rows_kernel<<<(p.n_envs + 7) / 8, 256, 0, st>>>(p, b, slots, rows, rows_f64, act);
+    return cudaGetLastError();
+}
+
 template <typename OT, bool STAB, bool SEL>
 static void expand_d(const ParamsT<DParams, SEL> &p, const BufParams &b, cudaStream_t st, unsigned g) {
     const bool small = p.W <= 16 && p.L <= 16 && p.H <= 16;  // the candidate key width of the step (launch_s)
@@ -483,6 +559,138 @@ cudaError_t launch_buffer_set_continuous(const CParams &p, const BufParams &b, c
     pctc_buf_set_kernel<<<(sel.n + 127) / 128, 128, 0, st>>>(ps, b, rows);
     expand_slots_c<true>(ps, b, st, sel.n);
     return cudaGetLastError();
+}
+
+// ---- buffered envs (pct_buffer_heuristic_actions; DESIGN.md section 22) ------------------------------------------------------------
+// One block per (env, slot), as pct_buf_expand_kernel: the selection for the slot's item on the env's state, written to the slot's BufHeurD.
+template <bool STAB, bool BIG>
+__global__ void __launch_bounds__(FEAS_THREADS, 4) pct_buf_heuristic_kernel(const DParams p, const HParams hp, const BufParams b) {
+    const int e = blockIdx.x / b.B;
+    const size_t s = (size_t)blockIdx.x;
+    const HeurPick r = heur_select<STAB, BIG>(p, hp, e, b.items + s * 4, &p.cold[e].lock);
+    if (threadIdx.x == 0) {
+        BufHeurD *o = (BufHeurD *)((BufSlotD *)b.scratch + s)->raw;
+        const int K = hp.code == PCT_H_MACS ? 4 : 1, R = p.setting == 2 ? 6 : 2;
+        o->score = r.score;
+        o->found = r.found;
+        o->rank = hp.code <= PCT_H_MACS ? r.c / (R * K) : 0;
+        o->lx = r.best.lx; o->ly = r.best.ly; o->sx = r.best.sx; o->sy = r.best.sy;
+    }
+}
+
+// Thread / env: the slot by the rules of DESIGN.md section 22 (best score in the heuristic's direction, OnlineBPH the lowest EMS rank, ties to
+// the lowest slot; RANDOM a uniform draw among the slots with a placement), its row, and LSAH's footprint of the chosen placement.  No slot
+// with a placement: slot 0 and the "no placement" row.
+__global__ void __launch_bounds__(128) pct_buf_heuristic_pick_kernel(const DParams p, const HParams hp, const BufParams b, int32_t *slots) {
+    const int e = blockIdx.x * 128 + threadIdx.x;
+    if (e >= p.n_envs) return;
+    const int code = hp.code, B = b.B;
+    const BufSlotD *sc = (const BufSlotD *)b.scratch + (size_t)e * B;
+    auto res = [&](int j) -> const BufHeurD & { return *(const BufHeurD *)sc[j].raw; };
+    int pick = -1;
+    if (code == PCT_H_RANDOM) {
+        int m = 0;
+        for (int j = 0; j < B; j++) m += res(j).found != 0;
+        if (m > 0) {
+            int k = (int)(rnd_u64(hp.seed ^ BUF_SLOT_SALT, (uint64_t)(p.env_id_base + e), (uint64_t)hp.t) % (uint64_t)m);
+            for (pick = 0; !res(pick).found || k-- > 0; pick++) {}
+        }
+    } else {
+        for (int j = 0; j < B; j++) {
+            const BufHeurD &r = res(j);
+            if (!r.found) continue;
+            bool take = pick < 0;
+            if (!take) {
+                const BufHeurD &q = res(pick);
+                if (code == PCT_H_ONLINEBPH) take = r.rank < q.rank;
+                else if (code == PCT_H_BR || code == PCT_H_MACS) take = r.score > q.score;
+                else take = r.score < q.score;
+            }
+            if (take) pick = j;
+        }
+    }
+    slots[e] = pick < 0 ? 0 : pick;
+    const BufHeurD &r = res(pick < 0 ? 0 : pick);
+    heur_row(hp.rows + (size_t)e * 9, pick >= 0, r.lx, r.ly, r.sx, r.sy);
+    if (pick >= 0 && code == PCT_H_LSAH) {
+        int32_t *s = hp.hstate + (size_t)e * 4;
+        const bool fresh = p.hot[e].h.n_box == 0;
+        lsah_note(s, fresh ? 0 : s[0], fresh ? 0 : s[1], fresh ? p.W : s[2], fresh ? p.L : s[3], r.lx, r.ly, r.sx, r.sy);
+    }
+}
+
+cudaError_t launch_buffer_heuristic_discrete(const DParams &p, const HParams &hp, const BufParams &b, int32_t *slots, cudaStream_t st) {
+    const unsigned g = (unsigned)p.n_envs * (unsigned)b.B;
+    if (heur_big(p, hp.code)) {
+        const size_t smem = heur_big_smem(p.W, p.L, p.setting == 2 ? 6 : 2);
+        if (p.setting == 2) pct_buf_heuristic_kernel<false, true><<<g, FEAS_THREADS, smem, st>>>(p, hp, b);
+        else pct_buf_heuristic_kernel<true, true><<<g, FEAS_THREADS, smem, st>>>(p, hp, b);
+    } else if (p.setting == 2) pct_buf_heuristic_kernel<false, false><<<g, FEAS_THREADS, 0, st>>>(p, hp, b);
+    else pct_buf_heuristic_kernel<true, false><<<g, FEAS_THREADS, 0, st>>>(p, hp, b);
+    pct_buf_heuristic_pick_kernel<<<(p.n_envs + 127) / 128, 128, 0, st>>>(p, hp, b, slots);
+    return cudaGetLastError();
+}
+
+
+// ---- buffered envs (pct_buffer_heuristic_actions_f64; DESIGN.md section 22): as pct_buf_heuristic_kernel / pct_buf_heuristic_pick_kernel ----
+template <bool STAB>
+__global__ void __launch_bounds__(64, STAB ? 8 : 12) pctc_buf_heuristic_kernel(const CParams p, const HParamsC hp, const BufParams b) {
+    const int e = blockIdx.x / b.B;
+    const size_t s = (size_t)blockIdx.x;
+    const HeurPickC r = heur_select_c<STAB>(p, hp, e, b.items + s * 4, &p.env[e].lock);
+    if (threadIdx.x == 0) {
+        BufHeurC *o = (BufHeurC *)&((BufSlotC *)b.scratch + s)->shuf[0][0];
+        o->score = r.score;
+        o->found = r.found;
+        o->rank = r.c / (p.setting == 2 ? 6 : 2);
+        o->lx = r.best.lx; o->ly = r.best.ly; o->sx = r.best.sx; o->sy = r.best.sy;
+    }
+}
+
+__global__ void __launch_bounds__(128) pctc_buf_heuristic_pick_kernel(const CParams p, const HParamsC hp, const BufParams b, int32_t *slots) {
+    const int e = blockIdx.x * 128 + threadIdx.x;
+    if (e >= p.n_envs) return;
+    const int code = hp.code, B = b.B;
+    const BufSlotC *sc = (const BufSlotC *)b.scratch + (size_t)e * B;
+    auto res = [&](int j) -> const BufHeurC & { return *(const BufHeurC *)&sc[j].shuf[0][0]; };
+    int pick = -1;
+    for (int j = 0; j < B; j++) {
+        const BufHeurC &r = res(j);
+        if (!r.found) continue;
+        bool take = pick < 0;
+        if (!take) {
+            const BufHeurC &q = res(pick);
+            if (code == PCT_H_ONLINEBPH) take = r.rank < q.rank;
+            else if (code == PCT_H_BR) take = r.score > q.score;
+            else take = r.score < q.score;
+        }
+        if (take) pick = j;
+    }
+    slots[e] = pick < 0 ? 0 : pick;
+    const BufHeurC &r = res(pick < 0 ? 0 : pick);
+    heur_row_c(hp.rows + (size_t)e * 9, pick >= 0, p.W, r.lx, r.ly, r.sx, r.sy);
+    if (pick >= 0 && code == PCT_H_LSAH) {
+        double *s = hp.hstate + (size_t)e * 4;
+        const bool fresh = p.env[e].h.n_box == 0;
+        lsah_note_c(s, fresh ? 0 : s[0], fresh ? 0 : s[1], fresh ? p.W : s[2], fresh ? p.L : s[3], r.lx, r.ly, r.sx, r.sy);
+    }
+}
+
+cudaError_t launch_buffer_heuristic_continuous(const CParams &p, const HParamsC &hp, const BufParams &b, int32_t *slots, cudaStream_t st) {
+    const unsigned g = (unsigned)p.n_envs * (unsigned)b.B;
+    if (p.setting == 2) pctc_buf_heuristic_kernel<false><<<g, 64, 0, st>>>(p, hp, b);
+    else pctc_buf_heuristic_kernel<true><<<g, 64, 0, st>>>(p, hp, b);
+    pctc_buf_heuristic_pick_kernel<<<(p.n_envs + 127) / 128, 128, 0, st>>>(p, hp, b, slots);
+    return cudaGetLastError();
+}
+
+// the dynamic shared memory limit of the BIG instantiations, as prepare_heuristic_big raises the plain kernel's (pct_create of a discrete handle
+// with W or L > 32; idempotent), so that launch_buffer_heuristic_discrete only enqueues
+cudaError_t prepare_buffer_heuristic_big() {
+    const int smem = (int)heur_big_smem(255, 255, 6);
+    cudaError_t e = cudaFuncSetAttribute(pct_buf_heuristic_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(pct_buf_heuristic_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    return e;
 }
 
 cudaError_t launch_buffer_items(const BufParams &b, int n_envs, const int32_t *env, int n, double *out, cudaStream_t st) {

@@ -67,6 +67,7 @@ struct pct_env_batch {
     int32_t *d_buf_nleaf = nullptr;  // [n_envs][B]
     int32_t *d_buf_l = nullptr;      // [n_envs]
     void *d_buf_scratch = nullptr;   // [n_envs][B] BufSlotD / BufSlotC
+    double *d_buf_rows = nullptr;    // [n_envs][9] the float64 action rows of pct_buffer_step_rows, as the apply kernel reads them
     uint64_t buf_snap_fp = 0;        // fingerprint of buffered snapshot records (snap_fp combined with B; pct_snapshot.cu)
     // staging for the host-buffer entry points
     void *d_obs = nullptr, *d_act = nullptr;

@@ -291,6 +291,7 @@ struct HParamsC {
 constexpr int HEUR_SIDE_MAX = 32;  // static height map of the heuristic kernel (HM / MACS / RANDOM above it: BIG instantiation); the single discrete query's limit
 cudaError_t launch_heuristic_discrete(const DParams &p, const HParams &hp, cudaStream_t st);
 cudaError_t prepare_heuristic_big();  // pct_create of a discrete handle with W or L > HEUR_SIDE_MAX
+bool heur_big(const DParams &p, int code);  // the launch takes the BIG instantiation (HM / MACS / RANDOM on a side > HEUR_SIDE_MAX)
 
 // batched placement queries (pct_query.cuh; continuous: pct_heuristics_continuous.cuh): row r asks k placements of env env[r]
 struct QParams {
@@ -427,5 +428,29 @@ cudaError_t launch_buffer_preview_continuous(const CParams &p, const ItemParams 
 cudaError_t launch_buffer_items(const BufParams &b, int n_envs, const int32_t *env, int n, double *out, cudaStream_t st);
 cudaError_t launch_buffer_policy_random(const BufParams &b, int n_envs, int nl, int64_t env_id_base, uint64_t seed, const int64_t *t_dev,
                                         int32_t *idx, cudaStream_t st);
+
+// heuristic baselines of buffered envs (pct_buffer_heuristic_actions*; pct_heuristics.cuh / pct_heuristics_continuous.cuh; DESIGN.md section 22).
+// The per-slot result of the selection kernel, in the slot's scratch (BufSlotD::raw / BufSlotC::shuf, which only the expansion uses), read by
+// the pick kernel of the same call.  rank: OnlineBPH's deep-bottom-left rank of the placement's EMS.
+struct BufHeurD {
+    long long score;
+    int32_t found, rank, lx, ly, sx, sy;
+};
+struct BufHeurC {
+    double score, lx, ly, sx, sy;
+    int32_t found, rank;
+};
+static_assert(sizeof(BufHeurD) <= sizeof(BufSlotD::raw) && sizeof(BufHeurC) <= sizeof(BufSlotC::shuf), "per-slot result in the slot's scratch");
+constexpr uint64_t BUF_SLOT_SALT = 0xB0FF510Full;  // RANDOM's slot draw: rnd_u64(seed ^ BUF_SLOT_SALT, env id, t)
+// the selection kernel over every (env, slot), then the pick kernel: slots[e] and row e of hp.rows; LSAH's footprint (hp.hstate)
+cudaError_t launch_buffer_heuristic_discrete(const DParams &p, const HParams &hp, const BufParams &b, int32_t *slots, cudaStream_t st);
+cudaError_t launch_buffer_heuristic_continuous(const CParams &p, const HParamsC &hp, const BufParams &b, int32_t *slots, cudaStream_t st);
+cudaError_t prepare_buffer_heuristic_big();  // with prepare_heuristic_big
+// the select kernel of pct_buffer_step_rows: slot slots[e] (outside [0, B): slot 0) becomes the env's item and leaf list, its row (outside: the
+// zero action) goes to act (n_envs x 9 float64, the apply kernel's actions), b.l[e] = slot * NL (the refill kernel's flat index)
+cudaError_t launch_buffer_select_rows_discrete(const DParams &p, const BufParams &b, const int32_t *slots, const void *rows, int rows_f64, double *act,
+                                               cudaStream_t st);
+cudaError_t launch_buffer_select_rows_continuous(const CParams &p, const BufParams &b, const int32_t *slots, const void *rows, int rows_f64,
+                                                 double *act, cudaStream_t st);
 
 }  // namespace pct

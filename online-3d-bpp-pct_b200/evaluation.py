@@ -45,9 +45,11 @@ def first_leaf_policy(obs, batch):
     return torch.zeros((obs.shape[0],), dtype=torch.int32, device=obs.device)
 
 
-def _streams(trajs, episodes, n_envs):
-    """(n_envs, (quota+1)*traj_len, 4) item streams: env e gets trajectories e+1, e+1+N, ... each padded with sentinels."""
-    traj_len = max(len(t) for t in trajs) + 1
+def _streams(trajs, episodes, n_envs, pad=1):
+    """(n_envs, (quota+1)*traj_len, 4) item streams: env e gets trajectories e+1, e+1+N, ... each padded with at least `pad` sentinels.
+    A buffered env (buffer=B) holds B draws at a time, so it needs pad = B: its last refills then draw sentinels and never reach into the next
+    trajectory (B = 1 is the plain env's padding)."""
+    traj_len = max(len(t) for t in trajs) + int(pad)
     quota = [(episodes - e + n_envs - 1) // n_envs for e in range(n_envs)]
     slots = max(quota) + 1  # one all-sentinel trajectory after the last real one: finished envs idle in 1-step episodes
     s = np.full((n_envs, slots, traj_len, 4), SENTINEL)
@@ -61,10 +63,12 @@ def _streams(trajs, episodes, n_envs):
 
 def evaluate_batched(data, setting, policy=None, container_size=(10, 10, 10), item_set=None, episodes=None, n_envs=1024,
                      continuous=False, LNES="EMS", internal_node_holder=80, leaf_node_holder=50, device=0, out_dir=None,
-                     sample_left_bound=None, max_steps=None):
+                     sample_left_bound=None, max_steps=None, buffer=None):
     """Runs `episodes` evaluation episodes (default: every trajectory but the first, like evaluation_episodes = len-1).
 
     policy(obs (N, obs_len) float32 CUDA tensor, batch) -> (N,) integer CUDA tensor of leaf indices.
+    buffer=B: buffered envs (PctBatch(..., buffer=B)) that hold B items of the trajectory at a time; the policy then returns flat leaf indices
+    j * NL + l into the leaves of all B items, as buffered_drl_gat does.
     Returns {'ratio': (episodes,) f64, 'length': (episodes,) int, 'packed': list of per-episode [[x,y,z,lx,ly,lz,0], ...],
              'result': the text of result.txt}; with `out_dir`, also writes trajs.npy and result.txt there
     (evaluation_tools.py:44-52).
@@ -78,7 +82,7 @@ def evaluate_batched(data, setting, policy=None, container_size=(10, 10, 10), it
     n = max(1, min(int(n_envs), episodes))
     if continuous:
         trajs = round3(trajs)
-    stream, traj_len, quota = _streams(trajs, episodes, n)
+    stream, traj_len, quota = _streams(trajs, episodes, n, pad=buffer or 1)
     policy = first_leaf_policy if policy is None else policy
     size_minimum = None
     if item_set is None:  # D:bin3D.py:23 takes min(item_set); a dataset run without one uses the smallest item of the data
@@ -86,7 +90,7 @@ def evaluate_batched(data, setting, policy=None, container_size=(10, 10, 10), it
     odt = torch.float64 if continuous else torch.float32  # float32 holds the discrete coordinates exactly
     batch = PctBatch(n, setting, container_size=container_size, item_set=item_set, internal_node_holder=internal_node_holder,
                      leaf_node_holder=leaf_node_holder, continuous=continuous, obs_dtype=odt, device=device, item_stream=stream,
-                     size_minimum=size_minimum, LNES=LNES)
+                     size_minimum=size_minimum, LNES=LNES, **({} if buffer is None else dict(buffer=buffer)))
     batch.set_trajectory_length(traj_len)
     nb = batch.nb
     binvol = float(container_size[0]) * float(container_size[1]) * float(container_size[2])
@@ -157,11 +161,12 @@ def main(argv=None):
     ap.add_argument("--num-envs", type=int, default=1024)
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--out-dir", default=None)
+    ap.add_argument("--buffer", type=int, default=None, help="buffered envs holding B items (the policy picks among the leaves of all of them)")
     a = ap.parse_args(argv)
     cs = a.container_size if a.continuous else [int(c) for c in a.container_size]
     out = evaluate_batched(a.dataset_path, a.setting, container_size=cs, episodes=a.evaluation_episodes, n_envs=a.num_envs,
                            continuous=a.continuous, LNES=a.lnes, internal_node_holder=a.internal_node_holder,
-                           leaf_node_holder=a.leaf_node_holder, device=a.device, out_dir=a.out_dir)
+                           leaf_node_holder=a.leaf_node_holder, device=a.device, out_dir=a.out_dir, buffer=a.buffer)
     print(out["result"])
 
 

@@ -7,6 +7,7 @@ order, scores and tie rules, and the ordinary step kernels apply them.  The summ
 heuristic.py returns: (mean utilisation, variance of utilisation, mean number of packed items).
 
     python -m pct_b200.heuristics --heuristic LSAH --setting 2 --evaluation-episodes 1000        (heuristic.py:579-610)
+    python -m pct_b200.heuristics --heuristic LSAH --setting 2 --evaluation-episodes 1000 --buffer 3   (online packing with a buffer of 3)
 """
 import numpy as np
 import torch
@@ -21,7 +22,7 @@ CONTINUOUS_HEURISTICS = ("LSAH", "OnlineBPH", "BR")  # tools.py:217-218
 
 def run_heuristic(name, setting, episodes, container_size=(10, 10, 10), item_set=None, data=None, n_envs=1024, seed=0, device=0,
                   internal_node_holder=80, leaf_node_holder=50, max_steps=None, return_episodes=False, continuous=False,
-                  sample_from_distribution=False, sample_left_bound=None, sample_right_bound=None, item_stream=None):
+                  sample_from_distribution=False, sample_left_bound=None, sample_right_bound=None, item_stream=None, buffer=None):
     """Plays `episodes` episodes of baseline `name` spread over min(n_envs, episodes) envs of one GPU batch.
 
     data=None: items are drawn on the fly from `item_set` (RandomBoxCreator) — or, continuous + sample_from_distribution, from
@@ -29,6 +30,8 @@ def run_heuristic(name, setting, episodes, container_size=(10, 10, 10), item_set
     data=path|list: the trajectory dataset of `--load-dataset` (LoadBoxCreator: episode k plays trajectory k+1).
     item_stream: (n, len, 3|4) per-env draw sequences instead (tests).
     continuous=True: PackingContinuous; only LSAH, OnlineBPH and BR (tools.py:217-218).
+    buffer=B: buffered envs holding B items; the baseline picks the item and its placement (buffer_heuristic_actions, DESIGN.md section 22).
+    With B = 1 the results are those without a buffer.
     -> (mean ratio, var ratio, mean length) like heuristic.py; with return_episodes also the per-episode arrays / packed lists.
     """
     if name not in _lib.HEURISTIC_CODES:
@@ -44,7 +47,7 @@ def run_heuristic(name, setting, episodes, container_size=(10, 10, 10), item_set
             trajs = round3(trajs)
         if not 0 < episodes <= len(trajs) - 1:
             raise ValueError("episodes must be in 1..len(dataset)-1")
-        stream, traj_len, quota = _streams(trajs, episodes, n)
+        stream, traj_len, quota = _streams(trajs, episodes, n, pad=buffer or 1)
     else:
         quota = np.array([(episodes - e + n - 1) // n for e in range(n)])
         if item_stream is not None:
@@ -54,7 +57,7 @@ def run_heuristic(name, setting, episodes, container_size=(10, 10, 10), item_set
     batch = PctBatch(n, setting, container_size=container_size, item_set=item_set, internal_node_holder=internal_node_holder,
                      leaf_node_holder=leaf_node_holder, obs_dtype=odt, seed=seed, device=device, item_stream=stream, continuous=continuous,
                      sample_from_distribution=sample_from_distribution, sample_left_bound=sample_left_bound,
-                     sample_right_bound=sample_right_bound)
+                     sample_right_bound=sample_right_bound, **({} if buffer is None else dict(buffer=buffer)))
     if traj_len:
         batch.set_trajectory_length(traj_len)
     nb = batch.nb
@@ -68,8 +71,12 @@ def run_heuristic(name, setting, episodes, container_size=(10, 10, 10), item_set
     while not (played >= quota).all() and t < limit:
         if prev is not None:
             prev.copy_(obs[:, :nb * 9])
-        rows = batch.heuristic_actions(name, seed=seed, t=t)
-        obs, _, done, info = batch.step(actions=rows)
+        if buffer is None:
+            rows = batch.heuristic_actions(name, seed=seed, t=t)
+            obs, _, done, info = batch.step(actions=rows)
+        else:
+            slots, rows = batch.buffer_heuristic_actions(name, seed=seed, t=t)
+            obs, _, done, info = batch.buffer_step_rows(slots, rows)
         t += 1
         done_h = done.cpu().numpy().astype(bool)
         who = np.nonzero(done_h & (played < quota))[0]
@@ -119,6 +126,7 @@ def main(argv=None):
     ap.add_argument("--container-size", type=float, nargs=3, default=None, help="givenData.container_size: [10,10,10]; continuous: [1,1,1]")
     ap.add_argument("--num-envs", type=int, default=1024)
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--buffer", type=int, default=None, help="online packing with a buffer: every env holds B items, the baseline picks one")
     a = ap.parse_args(argv)
     item_set = [(i, j, k) for i in range(1, 6) for j in range(1, 6) for k in range(1, 6)]  # givenData.py:7-14
     cs = a.container_size or ([1.0, 1.0, 1.0] if a.continuous else [10, 10, 10])  # givenData.py:4-5
@@ -129,7 +137,8 @@ def main(argv=None):
     mean, var, length = run_heuristic(a.heuristic, a.setting, a.evaluation_episodes, container_size=cs, item_set=item_set,
                                       data=a.dataset_path if a.load_dataset else None, n_envs=a.num_envs, device=a.device,
                                       continuous=a.continuous, sample_from_distribution=a.continuous,
-                                      sample_left_bound=0.1 if a.continuous else None, sample_right_bound=0.5 if a.continuous else None)
+                                      sample_left_bound=0.1 if a.continuous else None, sample_right_bound=0.5 if a.continuous else None,
+                                      buffer=a.buffer)
     print("The average space utilization:", mean)
     print("The variance of space utilization:", var)
     print("The average number of packed items:", length)
