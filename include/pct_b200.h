@@ -41,7 +41,19 @@ enum pct_status {
 
 enum pct_domain { PCT_DISCRETE = 0, PCT_CONTINUOUS = 1 };
 enum pct_obs_dtype { PCT_F32 = 0, PCT_F64 = 1 };
-enum pct_lnes { PCT_LNES_EMS = 0, PCT_LNES_EV = 1, PCT_LNES_EP = 2, PCT_LNES_CP = 3, PCT_LNES_FC = 4 };
+/* PCT_LNES_EV is the reference's EventPoint as the reference runs it: GENEMS only runs under 'EMS', so the ZMAP and the EMS list keep their
+ * reset values and EV offers the four bin corners per rotation at z = 0.  PCT_LNES_EVM (discrete only) is the same EventPoint with GENEMS
+ * run after every placement, as the reference behaves when its env is built with LNES='EMS' and Space.EMSPoint is rebound to EventPoint:
+ *   ZMAP   a pure function of the placed boxes in placement order.  Level 0: x_up {0}, y_left {0}, x_bottom {W}, y_right {L}.  A placed
+ *          box (x1,y1,z1,x2,y2,z2) adds to level z1: x2 to x_up if x2 < W, x1 to x_bottom, y2 to y_left if y2 < L, y1 to y_right; and if
+ *          z2 < H, to level z2 (created if new): x1 to x_up, y1 to y_left, x2 to x_bottom, y2 to y_right.  The lists are sorted sets; the
+ *          levels are ordered 0 first, then each new top height in placement order.
+ *   list   per level k that some EMS starts at (z == k), in level order: the CPython set of (xs, ys, k, xs + sx, ys + sy, k + sz) inserted
+ *          for each rotation, xs over x_up then x_bottom - sx, ys over y_left then y_right - sy; its tuples in set order that lie inside
+ *          an EMS of level k in x and y.  The levels' lists are concatenated; the keyed shuffle, the feasibility test and the leaf cap
+ *          follow as for every scheme.
+ *   PCT_FLAG_CAND_OVERFLOW  a level's set beyond 1228 entries (that level and the later ones are dropped) or the list beyond 1228. */
+enum pct_lnes { PCT_LNES_EMS = 0, PCT_LNES_EV = 1, PCT_LNES_EP = 2, PCT_LNES_CP = 3, PCT_LNES_FC = 4, PCT_LNES_EVM = 5 };
 /* heuristic baselines of the reference (heuristic.py): LASH :138-226, OnlineBPH :364-424, BR :500-577, MACS :11-131,
  * DBL :431-493, heightmap_min :232-293, random :300-357 */
 enum pct_heuristic {

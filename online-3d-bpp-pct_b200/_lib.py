@@ -23,7 +23,7 @@ class Config(C.Structure):
                 ("env_id_base", C.c_int64), ("no_auto_reset", C.c_int32), ("lnes", C.c_int32), ("shuffle", C.c_int32)]
 
 
-LNES_CODES = {"EMS": 0, "EV": 1, "EP": 2, "CP": 3, "FC": 4}
+LNES_CODES = {"EMS": 0, "EV": 1, "EP": 2, "CP": 3, "FC": 4, "EVM": 5}
 HEURISTIC_CODES = {"LSAH": 0, "OnlineBPH": 1, "BR": 2, "MACS": 3, "DBL": 4, "HM": 5, "RANDOM": 6}  # heuristic.py:593-606 names
 
 

@@ -127,8 +127,8 @@ int pct_create(const pct_config *cfg, int32_t n_envs, int32_t device, pct_handle
         g_create_err = "pct_create: holder sizes out of range (internal <= 80, leaf <= 64)";
         return PCT_ERR_INVALID;
     }
-    if (cfg->lnes < 0 || cfg->lnes > 4 || (cfg->lnes != 0 && cfg->domain != PCT_DISCRETE)) {
-        g_create_err = "pct_create: lnes must be 0 (EMS) .. 4 (FC); the continuous domain builds EMS only";
+    if (cfg->lnes < 0 || cfg->lnes > 5 || (cfg->lnes != 0 && cfg->domain != PCT_DISCRETE)) {
+        g_create_err = "pct_create: lnes must be 0 (EMS) .. 5 (EVM); the continuous domain builds EMS only";
         return PCT_ERR_INVALID;
     }
     if (cfg->domain == PCT_DISCRETE) {

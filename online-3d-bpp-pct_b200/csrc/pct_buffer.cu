@@ -332,6 +332,10 @@ __global__ void __launch_bounds__(BUF_THREADS) pct_buf_expand_kernel(const Param
             if (p.lnes == 0) {
                 const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, lane);
                 cand = cl.keys; n_cand = cl.n; fl = cl.flags;
+            } else if (p.lnes == 5) {
+                const CandList<SlotT> cl = gen_event_point_m<SlotT>(hot, rt, R, p.W, p.L, p.H, s.tabA, s.tabB, s.tabA,
+                                                                    sc->raw, out, lane);
+                cand = cl.keys; n_cand = cl.n; fl = cl.flags;
             } else {
                 uint32_t *raw = sc->raw;
                 RawList rl;

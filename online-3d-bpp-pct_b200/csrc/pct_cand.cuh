@@ -176,6 +176,184 @@ __device__ __noinline__ int gen_event_point(const RotTab *rt, int R, int W, int 
     return n;
 }
 
+// EventPoint over the maintained EMS list and ZMAP (LNES 'EVM', include/pct_b200.h): the reference's EventPoint (D:space.py:613-693) as it
+// behaves when GENEMS runs after every placement.  The ZMAP is a pure function of the placed boxes in order: level 0 holds x_up {0}, y_left
+// {0}, x_bottom {W}, y_right {L}; a box (x1,y1,z1,x2,y2,z2) adds x2 (if < W), y2 (if < L), x1, y1 to the four lists of level z1 and, if
+// z2 < H, x1, y1, x2, y2 to those of level z2, a level created in placement order.  The lists are sorted sets.  Per level with an EMS at
+// z == k, in level order: the CPython set of (xs, ys, k, xe, ye, k + sz) over rotation x {x_up, x_bottom - sx} x {y_left, y_right - sy},
+// then the tuples inside some EMS of that level (2-D containment).  The set emulation keys are offset coordinates (xs and ys may be
+// negative) with the rotation's canonical index; the kept tuples are written to `out` as candidate keys.  PCT_FLAG_CAND_OVERFLOW: a
+// level's set beyond the emulation's 1228 entries (the levels from it on are dropped) or the list beyond EVM_LIST_MAX (truncated).
+constexpr int EVM_LIST_MAX = 1228;
+
+__device__ __forceinline__ uint64_t py_int_hash(int v) { return (uint64_t)(int64_t)(v == -1 ? -2 : v); }
+
+// hash of the tuple a set key of level k stands for (noinline, as key_hash: it keeps the callers' register counts)
+template <int F>
+__device__ __noinline__ uint64_t evm_key_hash(uint32_t e, const RotTab *rt, int k) {
+    constexpr int OFF = 1 << (F - 1);
+    const int xs = (int)(e & ((1u << F) - 1)) - OFF, ys = (int)((e >> F) & ((1u << F) - 1)) - OFF, c = (int)(e >> (2 * F));
+    const uint64_t l[6] = {py_int_hash(xs), py_int_hash(ys), (uint64_t)k, py_int_hash(xs + rt->d[c][0]), py_int_hash(ys + rt->d[c][1]),
+                           (uint64_t)(k + rt->d[c][2])};
+    return tuple_hash6(l);
+}
+
+// the four ZMAP lists of level k, sorted, at lists[0 / 256 / 512 / 768]: x_up, y_left, x_bottom, y_right -> their lengths
+static __device__ __noinline__ int4 evm_level_lists(const int16_t (*box)[6], int n_box, int k, int W, int L, uint8_t *lists, int lane) {
+    // bitmasks over 0..255: lane = list * 8 + word
+    const int li = lane >> 3, lo = (lane & 7) * 32;
+    uint32_t bits = 0;
+    auto put = [&](int v) { if (v >= lo && v < lo + 32) bits |= 1u << (v - lo); };
+    if (k == 0) put(li == 0 || li == 1 ? 0 : li == 2 ? W : L);
+#pragma unroll 1
+    for (int i = 0; i < n_box; i++) {
+        const int16_t *b = box[i];
+        if (b[2] == k) {  // maintainEventBottom
+            if (li == 0) { if (b[3] < W) put(b[3]); } else if (li == 1) { if (b[4] < L) put(b[4]); } else put(b[li - 2]);
+        }
+        if (b[5] == k) put(li == 0 ? b[0] : li == 1 ? b[1] : b[li + 1]);  // AddNewEMSZ
+    }
+    const int cnt = __popc(bits);
+    int pre = cnt;  // inclusive prefix inside the list's 8 lanes
+#pragma unroll
+    for (int d = 1; d < 8; d <<= 1) {
+        const int t = __shfl_up_sync(FULL, pre, d);
+        if ((lane & 7) >= d) pre += t;
+    }
+    const int tot = __shfl_sync(FULL, pre, li * 8 + 7);
+    pre -= cnt;
+    for (uint32_t m = bits; m; m &= m - 1) lists[li * 256 + pre++] = (uint8_t)(lo + __ffs(m) - 1);
+    __syncwarp();
+    return make_int4(__shfl_sync(FULL, tot, 0), __shfl_sync(FULL, tot, 8), __shfl_sync(FULL, tot, 16), __shfl_sync(FULL, tot, 24));
+}
+
+// one level's set of set keys, inserted as build_candidates inserts: the table it ends in (a stage of tabA / tabB / tabBig) and its mask;
+// mask 0: the set outgrew the emulation, or a coordinate the key's range (PCT_FLAG_CAND_OVERFLOW)
+template <typename SlotT>
+struct EvmSet {
+    SlotT *tab;
+    uint32_t mask;
+};
+template <typename SlotT>
+__device__ __forceinline__ EvmSet<SlotT> evm_level_set(const RotTab *rt, int R, int k, const uint8_t *lists, int4 ln, SlotT *tabA, SlotT *tabB,
+                                                    SlotT *tabBig, int lane) {
+    constexpr int F = sizeof(SlotT) == 2 ? 6 : 10;          // set key fields: xs + OFF, ys + OFF, canonical rotation
+    constexpr int OFF = 1 << (F - 1);
+    constexpr SlotT EMPTY = (SlotT)~(SlotT)0;
+    const int nxu = ln.x, nyl = ln.y, ny = ln.y + ln.w, per = (ln.x + ln.z) * ny;
+    int nrot = 0;
+    for (int r = 0; r < R; r++) nrot += (rt->valid >> r) & 1;
+    const int raw_n = nrot * per;
+    auto hash_of = [rt, k](SlotT e) { return evm_key_hash<F>(e, rt, k); };
+    SlotT *tab = tabA;
+    uint32_t mask = 7;
+    int fill = 0;
+    if (lane < 8) tab[lane] = EMPTY;
+    __syncwarp();
+#pragma unroll 1
+    for (int base = 0; base < raw_n; base += 32) {
+        const int r = base + lane;
+        bool valid = false, range = false;
+        uint64_t hash = 0;
+        uint32_t key = 0xFFFFFFFFu;
+        if (r < raw_n) {
+            int q = r / per, rot = 0;
+            const int t = r - q * per, i = t / ny, j = t - i * ny;
+            for (; rot < R; rot++)
+                if (((rt->valid >> rot) & 1) && q-- == 0) break;
+            const int xs = i < nxu ? lists[i] : lists[512 + i - nxu] - rt->d[rot][0];
+            const int ys = j < nyl ? lists[256 + j] : lists[768 + j - nyl] - rt->d[rot][1];
+            range = xs + OFF < 0 || xs + OFF >= (1 << F) || ys + OFF < 0 || ys + OFF >= (1 << F);  // an item beyond the key's range
+            if (!range) {
+                valid = true;
+                key = (uint32_t)(xs + OFF) | ((uint32_t)(ys + OFF) << F) | ((uint32_t)rt->canon[rot] << (2 * F));
+                hash = hash_of((SlotT)key);
+            }
+        }
+        if (__any_sync(FULL, range)) return EvmSet<SlotT>{tab, 0};
+        const uint32_t same = __match_any_sync(FULL, key);
+        if (valid && (same & ((1u << lane) - 1))) valid = false;
+        SetProbe pr;
+        pr.home(hash, mask);
+#pragma unroll 1
+        for (;;) {
+            if (valid && set_seek(tab, mask, pr, [key](SlotT e) { return e == (SlotT)key; })) valid = false;
+            const uint32_t room = (mask * 3 + 4) / 5 - (uint32_t)fill;
+            const uint32_t cm = set_claim_round(valid, pr.slot(), lane, room);
+            if (!cm) break;
+            if ((cm >> lane) & 1) { tab[pr.slot()] = (SlotT)key; valid = false; }
+            fill += __popc(cm);
+            __syncwarp();
+            if ((uint32_t)fill * 5 >= mask * 3) {
+                uint32_t newsize = 8;
+                while (newsize <= (uint32_t)fill * 4) newsize <<= 1;
+                if (newsize > TAB_A) return EvmSet<SlotT>{tab, 0};
+                SlotT *nt = newsize == TAB_A ? tabBig : ((tab == tabA) ? tabB : tabA);
+                for (uint32_t t = lane; t < newsize; t += 32) nt[t] = EMPTY;
+                __syncwarp();
+                set_rehash(tab, mask, nt, newsize - 1, lane, hash_of);
+                tab = nt;
+                mask = newsize - 1;
+                pr.home(hash, mask);
+            }
+        }
+    }
+    __syncwarp();
+    return EvmSet<SlotT>{tab, mask};
+}
+
+template <typename SlotT>
+__device__ __noinline__ CandList<SlotT> gen_event_point_m(const DEnvHot *hot, const RotTab *rt, int R, int W, int L, int H, SlotT *tabA, SlotT *tabB,
+                                                          SlotT *tabBig, uint32_t *raw, SlotT *out, int lane) {
+    constexpr int KB = sizeof(SlotT) == 2 ? 4 : 8;          // candidate key fields (key_pack)
+    constexpr int F = sizeof(SlotT) == 2 ? 6 : 10;
+    constexpr int OFF = 1 << (F - 1);
+    constexpr SlotT EMPTY = (SlotT)~(SlotT)0;
+    const int16_t (*ems)[6] = hot->ems, (*box)[6] = hot->box;
+    const int n_ems = hot->h.n_ems, n_box = hot->h.n_box;
+    uint8_t *lists = (uint8_t *)raw;                        // x_up, y_left, x_bottom, y_right of the current level, 256 bytes each
+    int n_out = 0;
+#pragma unroll 1
+    for (int lv = -1; lv < n_box; lv++) {
+        // level keys: 0, then each top z2 < H not seen before, in placement order
+        int k = 0;
+        if (lv >= 0) {
+            k = box[lv][5];
+            bool seen = k >= H;
+            for (int i = lane; i < lv && !seen; i += 32) seen = box[i][5] == k;
+            if (__any_sync(FULL, seen)) continue;
+        }
+        bool has = false;
+        for (int i = lane; i < n_ems; i += 32) has |= ems[i][2] == k;
+        if (!__any_sync(FULL, has)) continue;
+        const EvmSet<SlotT> st = evm_level_set<SlotT>(rt, R, k, lists, evm_level_lists(box, n_box, k, W, L, lists, lane), tabA, tabB, tabBig, lane);
+        if (!st.mask) return CandList<SlotT>{out, n_out, PCT_FLAG_CAND_OVERFLOW};
+        // slot order, kept if inside an EMS of the level (D:space.py:676-691)
+#pragma unroll 1
+        for (uint32_t b2 = 0; b2 <= st.mask; b2 += 32) {
+            const uint32_t s = b2 + lane;
+            const SlotT e = s <= st.mask ? st.tab[s] : EMPTY;
+            bool keep = false;
+            int xs = 0, ys = 0, c = 0;
+            if (e != EMPTY) {
+                xs = (int)(e & ((1u << F) - 1)) - OFF; ys = (int)((e >> F) & ((1u << F) - 1)) - OFF; c = (int)(e >> (2 * F));
+                const int xe = xs + rt->d[c][0], ye = ys + rt->d[c][1];
+                for (int i = 0; i < n_ems && !keep; i++) {
+                    const int16_t *m = ems[i];
+                    keep = m[2] == k && m[0] <= xs && m[1] <= ys && xe <= m[3] && ye <= m[4];
+                }
+            }
+            const uint32_t km = __ballot_sync(FULL, keep);
+            const int p = n_out + __popc(km & ((1u << lane) - 1));
+            if (keep && p < EVM_LIST_MAX) out[p] = (SlotT)key_pack<KB>(xs, ys, k, c);
+            n_out += __popc(km);
+        }
+        __syncwarp();
+        if (n_out > EVM_LIST_MAX) return CandList<SlotT>{out, EVM_LIST_MAX, PCT_FLAG_CAND_OVERFLOW};
+    }
+    return CandList<SlotT>{out, n_out, 0};
+}
+
 // ExtremePoint2D (ep = true, D:space.py:696-750 + PctTools.extreme2D :107-135) and CornerPoint (ep = false,
 // D:space.py:752-806 + PctTools.corners2D :137-159): per distinct top level k, the 2-D points of the boxes whose top is
 // above k; points new w.r.t. the previous level x rotations.  Small serial algorithms over <= 80 boxes: lane 0 runs them.

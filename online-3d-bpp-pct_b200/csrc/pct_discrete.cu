@@ -490,8 +490,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kerne
             const int n_ems0 = h.n_ems;
             __syncwarp();
             int fl = 0;
-            // GENEMS only runs for LNES == 'EMS' (D:bin3D.py:172-175)
-            const int n_ems = p.lnes == 0 ? genems_warp(hot->ems, n_ems0, ems_tmp, ems_pk, b, p.low_bound, lane, fl) : n_ems0;
+            // GENEMS only runs for LNES == 'EMS' (D:bin3D.py:172-175); 'EVM' is EventPoint over the list it maintains
+            const int n_ems = (p.lnes == 0 || p.lnes == 5) ? genems_warp(hot->ems, n_ems0, ems_tmp, ems_pk, b, p.low_bound, lane, fl) : n_ems0;
             const double rw = (double)(nb0 * nb1 * nb2) / binvol * 10;  // D:bin3D.py:180-183
             reward = (float)rw;
             info.counter = n_box0 + 1;
@@ -540,7 +540,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K1_MINB) pct_apply_kerne
 // ---- K2: candidate leaves -----------------------------------------------------------------------------------
 // __grid_constant__ (K1, K2, emit): the __noinline__ phases take `const DParams &`; without it every thread first copies the 320 B parameter
 // block into its local-memory frame, so that the reference has an address, and reads the fields back from there.
-template <typename SlotT, bool BIGSM, bool SEL = false>
+// EVM: the LNES='EVM' instantiation (gen_event_point_m), kept apart so that the other schemes' instantiations keep their code and registers
+template <typename SlotT, bool BIGSM, bool SEL = false, bool EVM = false>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K2_MINB) pct_candidates_kernel(const __grid_constant__ ParamsT<DParams, SEL> p) {
     typedef Lay<SlotT, BIGSM> LY;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -590,7 +591,11 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, K2_MINB) pct_candidates_
     int fl = 0, n_cand = 0;
     SlotT *out = (SlotT *)cold->cand;
     constexpr int KB = sizeof(SlotT) == 2 ? 4 : 8;
-    if (p.lnes == 0) {
+    if constexpr (EVM) {
+        const CandList<SlotT> cl = gen_event_point_m<SlotT>(hot, rt, R, p.W, p.L, p.H, tabA, tabB,
+                                                            BIGSM ? tabA : (SlotT *)cold->tab_big, cold->raw, out, lane);
+        cand = cl.keys; n_cand = cl.n; fl = cl.flags;
+    } else if (p.lnes == 0) {
         const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, tabA, tabB, BIGSM ? tabA : (SlotT *)cold->tab_big, stg, lane);
         cand = cl.keys; n_cand = cl.n; fl = cl.flags;
     } else {
@@ -948,12 +953,14 @@ static cudaError_t launch_t(const ParamsT<DParams, SEL> &p_in, cudaStream_t st, 
         cudaError_t err = set_smem(pct_apply_kernel<STAB, false, SEL>, smem1);
         if (err == cudaSuccess && STAB) err = set_smem(pct_apply_kernel<STAB, STAB, SEL>, smem1);  // the ALIAS variant (stability settings only)
         if (err == cudaSuccess) err = set_smem(pct_candidates_kernel<SlotT, BIGSM, SEL>, smem2);
+        if (err == cudaSuccess) err = set_smem(pct_candidates_kernel<SlotT, BIGSM, SEL, true>, smem2);
         if (err != cudaSuccess) return err;
         attr_set = true;
     }
     int slots = p.n_envs;
     if constexpr (SEL) slots = p.sel.slots(p.n_envs);
     const int blocks = (slots + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+    auto *const k2 = p.lnes == 5 ? pct_candidates_kernel<SlotT, BIGSM, SEL, true> : pct_candidates_kernel<SlotT, BIGSM, SEL>;
     if (prof) cudaEventRecord(prof[0], st);
     if (apply) {
         if (STAB && (p.opt & PCT_OPT_ALIAS)) pct_apply_kernel<STAB, STAB, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem1, st>>>(p);
@@ -970,7 +977,7 @@ static cudaError_t launch_t(const ParamsT<DParams, SEL> &p_in, cudaStream_t st, 
         cudaLaunchConfig_t cfg{};
         cfg.stream = st; cfg.attrs = at; cfg.numAttrs = 1;
         cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(32 * WARPS_PER_BLOCK); cfg.dynamicSmemBytes = smem2;
-        err = cudaLaunchKernelEx(&cfg, pct_candidates_kernel<SlotT, BIGSM, SEL>, p);
+        err = cudaLaunchKernelEx(&cfg, k2, p);
         if (err != cudaSuccess) return err;
         if (k3_old) {
             cfg.gridDim = dim3(p.n_envs); cfg.blockDim = dim3(FEAS_THREADS); cfg.dynamicSmemBytes = 0;
@@ -979,7 +986,7 @@ static cudaError_t launch_t(const ParamsT<DParams, SEL> &p_in, cudaStream_t st, 
             if (err != cudaSuccess) return err;
         }
     } else {
-        pct_candidates_kernel<SlotT, BIGSM, SEL><<<blocks, 32 * WARPS_PER_BLOCK, smem2, st>>>(p);
+        k2<<<blocks, 32 * WARPS_PER_BLOCK, smem2, st>>>(p);
         if (prof) cudaEventRecord(prof[2], st);
         if (k3_old) {
             if (p.opt & PCT_OPT_DELTA) pct_feas_emit_kernel<OT, STAB, SlotT, true, SEL><<<slots, FEAS_THREADS, 0, st>>>(p);

@@ -77,6 +77,10 @@ __global__ void __launch_bounds__(EXPAND_THREADS) pct_expand_kernel(const DParam
             if (p.lnes == 0) {
                 const CandList<SlotT> cl = build_candidates<SlotT>(hot->ems, h.n_ems, rt, R, s.tabA, s.tabB, s.tabA, &s.stg, lane);
                 cand = cl.keys; n_cand = cl.n; fl = cl.flags;
+            } else if (p.lnes == 5) {
+                const CandList<SlotT> cl = gen_event_point_m<SlotT>(hot, rt, R, p.W, p.L, p.H, s.tabA, s.tabB, s.tabA,
+                                                                    cold->raw, out, lane);
+                cand = cl.keys; n_cand = cl.n; fl = cl.flags;
             } else {
                 uint32_t *raw = cold->raw;
                 RawList rl;

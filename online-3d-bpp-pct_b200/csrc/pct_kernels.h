@@ -220,7 +220,7 @@ struct DParams {
     float *reward;
     uint8_t *done;
     pct_step_info *info;
-    int lnes;  // leaf-node expansion scheme: 0 EMS, 1 EV, 2 EP, 3 CP, 4 FC
+    int lnes;  // leaf-node expansion scheme: 0 EMS, 1 EV, 2 EP, 3 CP, 4 FC, 5 EVM
     int shuffle;  // pct_config::shuffle: keyed permutation of the ordered candidate list (shuffle_candidates)
     int mode;  // 0 = reset all, 1 = step
     int keep_draw;      // mode 0: continue the item source instead of rewinding it (env.reset() after an episode)
